@@ -155,6 +155,14 @@ __global__ void k_bfs_popc(const uint32_t* bm, uint32_t words, unsigned long lon
   if (lane_id() == 0 && c) atomicAdd(out, c);
 }
 
+// rows with at least min_len entries
+__global__ void k_bfs_count_rows(const uint64_t* rp, uint32_t n, uint64_t min_len, unsigned long long* out) {
+  unsigned long long c = 0;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) c += rp[i + 1] - rp[i] >= min_len;
+  c = warp_sum(c);
+  if (lane_id() == 0 && c) atomicAdd(out, c);
+}
+
 // lid -> gid of every CSR entry / of the hub-neighbour table (global-frontier pull, several fragments)
 __global__ void k_bfs_gcol(const uint32_t* __restrict__ col, uint64_t m, uint32_t ivnum, uint32_t my_gid0,
                            const uint32_t* __restrict__ ovgid, uint32_t* gcol) {
@@ -268,15 +276,20 @@ k_bfs_hub_nbr(const uint64_t* __restrict__ rp, const uint64_t* __restrict__ row_
 // stand-alone kernel and the fused whole-query kernel.
 // ---------------------------------------------------------------------------
 constexpr uint32_t kPullSerialCap = 8;   // row entries a single thread probes
+constexpr uint32_t kListStage = 2048;    // tail-list entries a CTA gathers before one global append
 struct PullSmem {
   uint32_t v[kTileV];
   uint32_t lng[kTileV];   // candidates whose row is longer than the cap
   uint32_t nlong;
   uint32_t found[kTileV / 32];
   uint32_t words[kTB];
+  uint32_t cand[kTB];     // the ticket's candidate words, kept for the list append
   uint32_t warp[kTB / 32 + 1];
   uint32_t nz[kSuperTiles];
   uint32_t ticket;
+  // list append: staged entries [0, min(nstage, stage_full)), flushed with one atomic per CTA
+  uint32_t stage[kListStage];
+  uint32_t nstage, stage_full, stage_base;
 };
 
 struct PullArgs {
@@ -303,6 +316,17 @@ struct PullArgs {
   char* const* ship_send;
   const char* const* ship_recv;
   uint32_t ship_fid, ship_fnum, ship_off;
+  // Single-fragment fused kernel only (bfs_pull_phase<false, true>).  hub_first = 1: the adjacency is
+  // the hub-first shadow graph, so hub_nbr[v] is the first entry of v's sorted row (Setup fills it
+  // from there), the lids [0, sweep_v) are the non-isolated vertices and the lids [0, multi_v) the
+  // rows with two or more entries.  hub_first = 0: stage 2 scans whole rows and sweep_v = ivnum.
+  uint32_t hub_first;
+  uint32_t sweep_v, multi_v;
+  // Tail candidate list (hub-first order; list_cap = 0: none): once few non-isolated vertices are
+  // unvisited (BfsFusedArgs::list_gap), a pull level lists its unresolved candidates here; if they fit
+  // list_cap, every later level pulls over that list instead of the bitmap (bfs_list_pull)
+  uint32_t* list;
+  uint32_t list_cap;
 };
 
 // is vertex `id` in the frontier?  kGlobal is a compile-time switch: the single-fragment kernels
@@ -327,23 +351,36 @@ GL_DEV bool front_test(const PullArgs& a, const uint32_t* cur, uint32_t id) {
 // independent 16-byte loads in flight (stage 1), hands the unresolved ones to
 // a CTA-wide row scan (stage 2) and finally writes its visited / next-level
 // word with plain stores (the word belongs to this thread during the pull).
-template <bool kGlobal>
+// kTail (single-fragment fused kernel): the PullArgs hub_first fields apply,
+// and make_list appends the candidates left unresolved to a.list, counted in
+// ctrl->aux_ticket (the level that starts the tail, see bfs_list_pull).
+template <bool kGlobal, bool kTail = false>
 GL_DEV bool bfs_pull_phase(PullSmem& sm, const PullArgs& a,
                            const uint32_t* __restrict__ cur, uint32_t* vis,
-                           uint32_t* nxt, ScanCtrl* ctrl, ScanAcc& acc) {
+                           uint32_t* nxt, ScanCtrl* ctrl, ScanAcc& acc, bool make_list = false) {
   const uint32_t nwords = (a.ivnum + 31) / 32;
+  const bool hub_first = kTail && a.hub_first;
+  // hub-first order: entry 0 of a row is hub_nbr[v], which stage 1 has just tested
+  const uint32_t skip = hub_first ? 1u : 0u;
   uint64_t scanned = 0;
   uint32_t cand = 0;
   uint32_t st;
   bool shipped = false;
-  if (threadIdx.x == 0) sm.nlong = 0;
+  if (threadIdx.x == 0) {
+    sm.nlong = 0;
+    if (kTail) {
+      sm.nstage = 0;
+      sm.stage_full = kListStage;
+    }
+  }
   __syncthreads();
-  while (next_super_tile(sm, &ctrl->tile_ticket, a.ivnum,
+  while (next_super_tile(sm, &ctrl->tile_ticket, kTail ? a.sweep_v : a.ivnum,
                          [&](uint32_t w) { return a.nz[w] & ~vis[w]; }, &st)) {
     const uint32_t word = sm.words[threadIdx.x];
     const uint32_t wi = st * (kSuperV / 32) + threadIdx.x;
     const uint32_t vbase = wi * 32;
     sm.words[threadIdx.x] = 0;  // reused as the stage-2 result word
+    if (kTail && make_list) sm.cand[threadIdx.x] = word;
     // ---- stage 1 ----
     uint32_t res = 0;
     if (word) {
@@ -376,6 +413,10 @@ GL_DEV bool bfs_pull_phase(PullSmem& sm, const PullArgs& a,
     }
     // ---- stage 2: leftovers scan their row, kTileV candidates per pass ----
     uint32_t rest = word & ~res;
+    if (hub_first) {
+      // a row of one entry has nothing left to scan: only lids below multi_v enter stage 2
+      rest &= vbase + 32 <= a.multi_v ? 0xFFFFFFFFu : (vbase >= a.multi_v ? 0u : (1u << (a.multi_v - vbase)) - 1u);
+    }
     uint32_t total;
     uint32_t off = block_excl_scan(__popc(rest), sm.warp, &total);
     cand += (threadIdx.x == 0) ? total : 0;
@@ -411,7 +452,7 @@ GL_DEV bool bfs_pull_phase(PullSmem& sm, const PullArgs& a,
           vv[k] = i < nc ? sm.v[i] : kInfU32;
         }
 #pragma unroll
-        for (int k = 0; k < kIL; ++k) bb[k] = vv[k] != kInfU32 ? a.rp[vv[k]] : 0ull;
+        for (int k = 0; k < kIL; ++k) bb[k] = vv[k] != kInfU32 ? a.rp[vv[k]] + skip : 0ull;
         uint32_t act = 0, foundm = 0;
 #pragma unroll
         for (int k = 0; k < kIL; ++k) {
@@ -450,7 +491,7 @@ GL_DEV bool bfs_pull_phase(PullSmem& sm, const PullArgs& a,
       const uint32_t nl = sm.nlong;
       for (uint32_t i = threadIdx.x >> 5; i < nl; i += kTB / 32) {
         const uint32_t v = sm.lng[i];
-        const uint64_t b = a.rp[v];
+        const uint64_t b = a.rp[v] + skip;
         const uint32_t len = (uint32_t) (a.row_end[v] - b);
         const uint32_t* row = a.col + b;
         bool hit = false;
@@ -486,7 +527,36 @@ GL_DEV bool bfs_pull_phase(PullSmem& sm, const PullArgs& a,
       }
     }
     acc.next_count += __popc(found_w);
+    if (kTail && make_list) {
+      // the candidates still unresolved become the tail list: staged in shared memory (a global
+      // atomic per warp and ticket, all on one address, cost more than the level's whole pull);
+      // a warp whose entries do not fit any more appends them to the list itself
+      uint32_t surv = sm.cand[threadIdx.x] & ~found_w;
+      const uint32_t ns = __popc(surv);
+      const uint32_t incl = warp_incl_scan(ns);
+      uint32_t at = 0;
+      if (lane_id() == 31 && incl) {
+        at = atomicAdd(&sm.nstage, incl);
+        if (at + incl > kListStage) {
+          atomicMin(&sm.stage_full, at);   // the staged entries stay a prefix
+          at = kListStage + atomicAdd(&ctrl->aux_ticket, incl);
+        }
+      }
+      at = __shfl_sync(0xffffffffu, at, 31) + incl - ns;
+      for (; surv; surv &= surv - 1, ++at) {
+        const uint32_t v = vbase + __ffs(surv) - 1;
+        if (at < kListStage) sm.stage[at] = v;
+        else if (at - kListStage < a.list_cap) a.list[at - kListStage] = v;
+      }
+    }
     __syncthreads();
+  }
+  if (kTail && make_list) {
+    const uint32_t n = sm.nstage < sm.stage_full ? sm.nstage : sm.stage_full;
+    if (threadIdx.x == 0 && n) sm.stage_base = atomicAdd(&ctrl->aux_ticket, n);
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < n; i += kTB)
+      if (sm.stage_base + i < a.list_cap) a.list[sm.stage_base + i] = sm.stage[i];
   }
   acc.touched = acc.next_count;
   unsigned long long s = warp_sum((unsigned long long) scanned);
@@ -502,6 +572,71 @@ k_bfs_pull(PullArgs a, const uint32_t* __restrict__ cur, uint32_t* vis,
   ScanAcc acc;
   bfs_pull_phase<false>(sm, a, cur, vis, nxt, ctrl, acc);
   flush_acc(acc, ctrl);
+}
+
+// Tail pull level (single fragment, hub-first order): the candidates are the
+// list[0, n) that an earlier pull level left unresolved -- not a sweep of the
+// whole bitmap.  One entry per thread, grid-stride, no tickets and no CTA
+// barriers: hub probe, then the row from entry 1 (entry 0 is hub_nbr[v]);
+// rows longer than 1 + kPullSerialCap are finished by their warp, 32 entries
+// per step.  Words are shared between threads here, so hits set vis / nxt
+// with atomicOr.  A resolved entry is overwritten with kInfU32 in place: the
+// list is not compacted (no atomic round trip per level; in the tail few
+// entries resolve per level, and a dead entry costs one coalesced load).
+GL_DEV void bfs_list_pull(const PullArgs& a, const uint32_t* __restrict__ cur, uint32_t* vis, uint32_t* nxt,
+                          uint32_t n, ScanCtrl* ctrl, ScanAcc& acc) {
+  uint32_t* list = a.list;
+  const uint32_t lane = lane_id();
+  uint64_t scanned = 0;
+  uint32_t cand = 0;
+  for (uint32_t base = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; base < n; base += gridDim.x * blockDim.x) {
+    const uint32_t i = base + lane;
+    const uint32_t v = i < n ? list[i] : kInfU32;
+    bool hit = false;
+    uint64_t b = 0;
+    uint32_t len = 0;
+    if (v != kInfU32) {
+      const uint32_t h = a.hub_nbr[v];
+      b = a.rp[v] + 1;
+      const uint64_t e = a.row_end[v];
+      hit = h != kInfU32 && front_test<false>(a, cur, h);
+      len = e > b ? (uint32_t) (e - b) : 0u;
+      const uint32_t serial = len < kPullSerialCap ? len : kPullSerialCap;
+      ++cand;
+      ++scanned;
+      for (uint32_t p = 0; p < serial && !hit; ++p, ++scanned) hit = front_test<false>(a, cur, a.col[b + p]);
+    }
+    for (uint32_t lng = __ballot_sync(0xffffffffu, !hit && len > kPullSerialCap); lng; lng &= lng - 1) {
+      const int src = __ffs(lng) - 1;
+      const uint64_t lb = __shfl_sync(0xffffffffu, b, src);
+      const uint32_t llen = __shfl_sync(0xffffffffu, len, src);
+      bool found = false;
+      uint32_t p = kPullSerialCap;
+      for (; p < llen; p += 32) {
+        const uint32_t q = p + lane;
+        if (__any_sync(0xffffffffu, q < llen && front_test<false>(a, cur, a.col[lb + q]))) {
+          found = true;
+          p += 32;
+          break;
+        }
+      }
+      if (lane == (uint32_t) src) {
+        hit = found;
+        scanned += (p < llen ? p : llen) - kPullSerialCap;
+      }
+    }
+    if (hit) {
+      atomicOr(vis + (v >> 5), 1u << (v & 31));
+      atomicOr(nxt + (v >> 5), 1u << (v & 31));
+      list[i] = kInfU32;
+      acc.next_count++;
+    }
+  }
+  acc.touched = acc.next_count;
+  const unsigned long long s = warp_sum((unsigned long long) scanned);
+  const uint32_t c = warp_sum(cand);
+  if (lane == 0 && s) atomicAdd(&ctrl->scanned, s);
+  if (lane == 0 && c) atomicAdd(&ctrl->frontier, (unsigned long long) c);
 }
 
 // ---------------------------------------------------------------------------
@@ -556,7 +691,9 @@ GL_DEV unsigned long long global_ns() {
 // pull -> push (for good) when the frontier shrinks below V/24 (Beamer et
 // al.; the reference uses vertex ratios, bfs.h:171-180 — the schedule only
 // affects speed, never the levels).  phase: 0 = initial push, 1 = pull,
-// 2 = final push.
+// 2 = final push; k_bfs_fused adds kListPull = pull over the tail candidate
+// list, kept until the query ends (never an input of bfs_next_phase).
+constexpr uint32_t kListPull = 3;
 GL_DEV uint32_t bfs_next_phase(uint32_t phase, unsigned long long n_f,
                                unsigned long long m_f, unsigned long long m_u,
                                uint32_t ivnum, int direction_opt, uint32_t beta,
@@ -568,17 +705,41 @@ GL_DEV uint32_t bfs_next_phase(uint32_t phase, unsigned long long n_f,
     // ~ the frontier's edges plus two grid barriers: keep pulling while the
     // frontier is large (Beamer) or while few candidates remain per frontier
     // vertex (the tail of a skewed graph); go back to push for long sparse tails.
-    if (n_f >= (unsigned long long) ivnum / beta) return 1u;
+    // n_f >= floor(ivnum / beta), without a division the compiler would hoist out of the level loop
+    // and keep live (k_bfs_fused has no register to spare)
+    if ((n_f + 1) * beta > ivnum) return 1u;
     return unvisited_nz <= 64ull * n_f ? 1u : 2u;
   }
   return 2u;
 }
 
+// seed_hubs (k_bfs_fused): a source row longer than hub_deg is cut into its hub work items here,
+// by the whole block, so that level 0 is the hub phase alone (no frontier sweep, one grid.sync fewer)
 __global__ void k_bfs_seed_fused(uint32_t src, int has_src, uint32_t* lv0,
                                  uint32_t* vis, const uint64_t* rp,
-                                 unsigned long long m_total, BfsFusedCtl* ctl) {
-  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+                                 unsigned long long m_total, BfsFusedCtl* ctl,
+                                 int seed_hubs = 0, HubItem* hubs = nullptr, uint32_t hub_cap = 0, uint32_t hub_deg = 0) {
+  if (blockIdx.x != 0) return;
+  uint32_t pieces = 0;
+  if (seed_hubs && has_src) {
+    const uint64_t b = rp[src], e = rp[src + 1];
+    if (e - b > hub_deg) {
+      pieces = (uint32_t) ((e - b + kHubChunk - 1) / kHubChunk);
+      for (uint32_t p = threadIdx.x; p < pieces && p < hub_cap; p += blockDim.x) {
+        HubItem it;
+        it.v = src;
+        it.pad = 0;
+        it.begin = b + (uint64_t) p * kHubChunk;
+        it.end = (it.begin + kHubChunk < e) ? it.begin + kHubChunk : e;
+        hubs[p] = it;
+      }
+    }
+  }
+  if (threadIdx.x != 0) return;
   ctl->c[0] = ScanCtrl();
+  // as the frontier sweep of level 0 would have left them: the source expanded, its row listed
+  ctl->c[0].hub_count = pieces;
+  ctl->c[0].frontier = pieces ? 1 : 0;
   ctl->c[1] = ScanCtrl();
   ctl->c[2] = ScanCtrl();
   ctl->levels = 0;
@@ -652,6 +813,9 @@ struct BfsFusedArgs {
   uint32_t hub_cap, hub_deg;
   int hub_tma;       // hub phase staged through the TMA engine (GL_HUB_TMA=0: plain loads)
   const uint8_t* deg8;   // byte-sized degree classes for the frontier-edge statistic (OpBfsPush)
+  uint32_t push_v;       // push levels sweep the frontier over lids [0, push_v)
+  unsigned long long m_total;   // CSR entries of the graph (the push -> pull rule)
+  uint32_t list_gap;             // pull levels try the tail list once at most this many vertices are unvisited
 };
 
 // Level d reads lv[d] and writes lv[d+1] (pre-zeroed).  Every thread derives
@@ -672,21 +836,22 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
   unsigned long long n_f = ctl->r_nf;
   unsigned long long m_f = ctl->r_mf;
   unsigned long long visited_edges = ctl->r_visited_edges;
-  const unsigned long long m_total = ctl->m_total;
+  const unsigned long long m_total = a.m_total;   // a kernel parameter: no register held across the levels
   unsigned long long visited_cnt = ctl->r_visited_cnt;
   uint32_t phase = ctl->r_phase;
   if (phase == 0xFFFFFFFFu)
     phase = bfs_next_phase(0, n_f, m_f, m_total - visited_edges, a.pa.ivnum, a.direction_opt, a.beta, a.nz_total);
   for (uint32_t depth = 0; n_f != 0; ++depth) {
     if (depth + 1 >= a.max_lv) {
-      // ring full: park the state; the host spills levels [0, max_lv-1) and relaunches
+      // ring full: park the state; the host spills levels [0, max_lv-1) and relaunches (the tail
+      // list does not survive the relaunch: its first level sweeps the bitmap again)
       if (gtid == 0) {
         ctl->overflow = 1;
         ctl->p_nf = n_f;
         ctl->p_mf = m_f;
         ctl->p_visited_edges = visited_edges;
         ctl->p_visited_cnt = visited_cnt;
-        ctl->p_phase = phase;
+        ctl->p_phase = phase == kListPull ? 1u : phase;
       }
       break;
     }
@@ -694,20 +859,35 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
     const uint32_t* cur = a.lv + (size_t) depth * a.words;
     uint32_t* nxt = a.lv + (size_t) (depth + 1) * a.words;
     ScanAcc acc;
-    if (phase != 1) {
+    // A pull level lists its unresolved candidates once at most list_gap (> list_cap) non-isolated
+    // vertices are unvisited: most of them are usually found by that level, and a list that comes out
+    // longer than list_cap is simply not used (the next level sweeps the bitmap and tries again; the
+    // attempt costs shared-memory appends).  The list's length travels from level to level in
+    // C->aux_ticket.
+    if (phase == kListPull) {
+      const uint32_t n = ((const volatile ScanCtrl*) &ctl->c[(depth + 2) % 3])->aux_ticket;
+      if (gtid == 0) C->aux_ticket = n;
+      bfs_list_pull(a.pa, cur, a.vis, nxt, n, C, acc);
+    } else if (phase == 1) {
+      bfs_pull_phase<false, true>(sm.pull, a.pa, cur, a.vis, nxt, C, acc,
+                                  a.pa.list_cap && a.nz_total <= visited_cnt + a.list_gap);
+    } else {
       OpBfsPush op{a.vis, nxt, nullptr, a.er.rp, a.pa.ivnum, a.deg8};
-      frontier_scan_phase<OpBfsPush>(sm.scan, cur, a.pa.ivnum, a.er, op, C, a.hubs, a.hub_cap, a.hub_deg, acc);
-      grid.sync();
+      // level 0 of a query whose seed listed the source row's hub items: nothing else to sweep for
+      if (depth != 0 || ((const volatile ScanCtrl*) C)->hub_count == 0) {
+        frontier_scan_phase<OpBfsPush>(sm.scan, cur, a.push_v, a.er, op, C, a.hubs, a.hub_cap, a.hub_deg, acc);
+        grid.sync();
+      }
       if (a.hub_tma) hub_scan_phase_tma<OpBfsPush>(sm.hub, a.er, op, C, a.hubs, a.hub_cap, acc);
       else hub_scan_phase<OpBfsPush>(&s_item, a.er, op, C, a.hubs, a.hub_cap, acc);
-    } else {
-      bfs_pull_phase<false>(sm.pull, a.pa, cur, a.vis, nxt, C, acc);
     }
     flush_acc(acc, C);
     grid.sync();
     const volatile ScanCtrl* VC = C;
     const unsigned long long next_count = VC->next_count;
     const unsigned long long next_edges = VC->next_edges;
+    const bool listed = (phase == kListPull || (phase == 1 && a.pa.list_cap && a.nz_total <= visited_cnt + a.list_gap)) &&
+                        VC->aux_ticket <= a.pa.list_cap;
     if (gtid == 0) {
       const uint32_t adepth = a.depth_base + depth;
       if (adepth < (uint32_t) kMaxFusedStats) {
@@ -715,22 +895,25 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
         ls.t_ns = global_ns();
         ls.scanned = VC->scanned;
         ls.frontier = (uint32_t) (n_f > 0xFFFFFFFFull ? 0xFFFFFFFFull : n_f);
-        ls.mode = phase == 1 ? 1u : 0u;
+        ls.mode = (phase == 1 || phase == kListPull) ? 1u : 0u;
         ctl->stat[adepth] = ls;
       }
       ctl->levels = adepth + 1;
       ctl->touched += VC->touched;
-      // c[(depth+2)%3] was last read right after the previous level's barrier
+      // c[(depth+2)%3] was last read during this level
       ctl->c[(depth + 2) % 3] = ScanCtrl();
     }
     n_f = next_count;
     m_f = next_edges;
     visited_edges += next_edges;
     visited_cnt += next_count;
-    phase = bfs_next_phase(phase, n_f, m_f,
-                           m_total > visited_edges ? m_total - visited_edges : 0,
-                           a.pa.ivnum, a.direction_opt, a.beta,
-                           a.nz_total > visited_cnt ? a.nz_total - visited_cnt : 0);
+    // while a list is in use the level costs O(list) and one grid.sync: keep pulling (depths are the
+    // same in either direction)
+    phase = listed ? kListPull
+                   : bfs_next_phase(phase, n_f, m_f,
+                                    m_total > visited_edges ? m_total - visited_edges : 0,
+                                    a.pa.ivnum, a.direction_opt, a.beta,
+                                    a.nz_total > visited_cnt ? a.nz_total - visited_cnt : 0);
   }
 }
 
@@ -1355,6 +1538,12 @@ struct BfsApp : gl_app {
   bool global_front = false;
   uint32_t *perm = nullptr, *order = nullptr, *nz_p = nullptr, *col_p = nullptr;
   uint64_t* rp_p = nullptr;
+  // one fragment in hub-first order: rows of two or more entries are lids [0, multi_v); the fused
+  // kernel's tail candidate list (kTailList entries)
+  static constexpr uint32_t kTailList = 1u << 16;
+  static constexpr uint32_t kListTry = 16;   // the list is tried from kListTry x kTailList unvisited vertices on
+  uint32_t multi_v = 0;
+  uint32_t* tail_list = nullptr;
   uint32_t src_ = 0;
   int has_src_ = 0;
   unsigned long long nz_total = 0, visited_cnt = 0;
@@ -1385,6 +1574,7 @@ struct BfsApp : gl_app {
     cudaFree(nz_p);
     cudaFree(col_p);
     cudaFree(rp_p);
+    cudaFree(tail_list);
     cudaFree(nz_in);
     cudaFree(gcol);
     cudaFree(hub_nbr_g);
@@ -1456,14 +1646,27 @@ struct BfsApp : gl_app {
       if (fv.ivnum) GL_LAUNCH(k_bfs_nz, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, fv.ivnum, nz_in);
       g_nz = nz_in;   // pull candidates / "still reachable" statistics: in-degree > 0
     }
-    if (fv.ivnum && can_pull())
-      GL_LAUNCH(k_bfs_hub_nbr, eng.sm_count * 8, 256, eng.stream, p_rp, row_end(), p_col, fv.ivnum, hub_nbr);
+    if (fv.ivnum && can_pull()) {
+      // hub-first order: the first entry of a sorted row is its highest-degree neighbour, and the pull
+      // relies on hub_nbr[v] being that entry (stage 2 starts after it)
+      if (perm) GL_LAUNCH(k_bfs_first_col, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, p_col, fv.ivnum, hub_nbr);
+      else GL_LAUNCH(k_bfs_hub_nbr, eng.sm_count * 8, 256, eng.stream, p_rp, row_end(), p_col, fv.ivnum, hub_nbr);
+    }
     {
       unsigned long long* d_cnt = nullptr;
-      GL_CUDA(cudaMalloc(&d_cnt, 8));
-      GL_CUDA(cudaMemsetAsync(d_cnt, 0, 8, eng.stream));
+      GL_CUDA(cudaMalloc(&d_cnt, 16));
+      GL_CUDA(cudaMemsetAsync(d_cnt, 0, 16, eng.stream));
       GL_LAUNCH(k_bfs_popc, eng.sm_count * 4, 256, eng.stream, g_nz, (uint32_t) bm_words(fv.ivnum), d_cnt);
       GL_CUDA(cudaMemcpyAsync(&nz_total, d_cnt, 8, cudaMemcpyDeviceToHost, eng.stream));
+      if (perm) {
+        // descending degree: the rows of two or more entries are a prefix of the lids
+        unsigned long long m2 = 0;
+        GL_LAUNCH(k_bfs_count_rows, eng.sm_count * 4, 256, eng.stream, p_rp, fv.ivnum, (uint64_t) 2, d_cnt + 1);
+        GL_CUDA(cudaMemcpyAsync(&m2, d_cnt + 1, 8, cudaMemcpyDeviceToHost, eng.stream));
+        GL_CUDA(cudaStreamSynchronize(eng.stream));
+        multi_v = (uint32_t) m2;
+        GL_CUDA(cudaMalloc(&tail_list, sizeof(uint32_t) * kTailList));
+      }
       GL_CUDA(cudaStreamSynchronize(eng.stream));
       cudaFree(d_cnt);
     }
@@ -1664,8 +1867,8 @@ struct BfsApp : gl_app {
     uint32_t src = 0;
     int has_src = has_src_;
     src = src_;   // already translated to the hub-first rank in Setup
-    GL_LAUNCH(k_bfs_seed_fused, 1, 32, s, src, has_src, level_bm(0), vis, g_rp,
-              (unsigned long long) g_m_total, d_ctl);
+    GL_LAUNCH(k_bfs_seed_fused, 1, 256, s, src, has_src, level_bm(0), vis, g_rp,
+              (unsigned long long) g_m_total, d_ctl, fv.fnum == 1 ? 1 : 0, eng.hubs, eng.hub_cap, eng.hub_deg);
     BfsFusedArgs a;
     a.pa = pull_args();
     a.er = EdgeRange{g_rp, g_col, nullptr};
@@ -1676,6 +1879,7 @@ struct BfsApp : gl_app {
     a.direction_opt = can_pull() ? 1 : 0;
     a.beta = cfg.reserved[2] > 0 ? (uint32_t) cfg.reserved[2] : 24u;
     a.nz_total = nz_total;
+    a.m_total = g_m_total;
     a.ctl = d_ctl;
     a.hubs = eng.hubs;
     a.hub_cap = eng.hub_cap;
@@ -1685,6 +1889,16 @@ struct BfsApp : gl_app {
     // k_hub_scan_tma is the default elsewhere
     a.hub_tma = (getenv("GL_HUB_TMA") && atoi(getenv("GL_HUB_TMA")) == 2) ? 1 : 0;
     const bool multi = fv.fnum > 1;
+    // one fragment in hub-first order: the vertices with edges are lids [0, nz_total), so the sweeps
+    // stop there (a push level also covers an isolated source)
+    const bool hub_first = perm && !multi;
+    a.pa.hub_first = hub_first ? 1u : 0u;
+    a.pa.sweep_v = hub_first ? (uint32_t) nz_total : fv.ivnum;
+    a.pa.multi_v = hub_first ? multi_v : 0u;
+    a.push_v = hub_first ? std::min<uint32_t>(fv.ivnum, std::max<uint32_t>((uint32_t) nz_total, src + 1)) : fv.ivnum;
+    a.pa.list = hub_first ? tail_list : nullptr;
+    a.pa.list_cap = hub_first ? kTailList : 0u;
+    a.list_gap = kListTry * kTailList;
     if (!fused_grid)
       fused_grid = multi ? (global_front ? persistent_grid(k_bfs_fused_multi<true>, eng.sm_count)
                                          : persistent_grid(k_bfs_fused_multi<false>, eng.sm_count))
