@@ -327,7 +327,11 @@ void orc_pagerank(void* h, double delta, int max_round, int mode,
   const int64_t n = g->n;
   const Csr& oe = g->out;
   const Csr& ie = g->directed ? g->in : g->out;
-  if (max_round <= 0 && mode != 1) {
+  // max_round <= 0: pagerank.h:52-55 returns from PEval before it writes a
+  // rank, so the CPU app prints its zero-initialised result; modes 1 and 2 run
+  // their initialisation and return 1/N (pagerank_parallel.h:108-116 multiplies
+  // the PEval values p/deg back by the degree in the first IncEval).
+  if (max_round <= 0 && mode == 0) {
     for (int64_t v = 0; v < n; ++v) rank[v] = 0;
     return;
   }

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Regenerates tests/golden/ref_outputs.{json,npz}: what the reference's CPU
 apps (oracle/_ref/ref_driver, built by `make -C oracle ref` from the reference
-sources) compute on the inputs of tests/test_ref_golden.py, test_rmat_def.py
-and test_gpu_fullsize.py.  Those tests compare with the stored results, so they
+sources) compute on the inputs of tests/test_ref_golden.py, test_rmat_def.py,
+test_shapes_oracle.py and test_gpu_fullsize.py.  Those tests compare with the stored results, so they
 run where the reference is not installed.
 
 Exact results are stored as digests (golden_io.digest; WCC labels after
@@ -21,6 +21,7 @@ sys.path.insert(0, ROOT)
 
 from oracle import pyoracle, refdriver  # noqa: E402
 from tests import golden_io as G  # noqa: E402
+from tests import shapes  # noqa: E402
 from tests.test_gpu_fullsize import REF_SCALE, pagerank_sample_index  # noqa: E402
 from tests.test_ref_golden import _random_graph  # noqa: E402
 from tests.test_rmat_def import RMAT_CASES  # noqa: E402
@@ -81,6 +82,16 @@ for scale, seed, wmode in RMAT_CASES:
     if wmode:
         e["w"] = G.digest(raw[2 * m:].view(np.float64))
     out["rmat_edges"]["%d,%d,%d" % (scale, seed, wmode)] = e
+
+# test_shapes_oracle.py: PageRank after 0 and 1 rounds on a star (undirected) and on a
+# directed star into a sink, from both CPU PageRank apps of the reference
+for name, (n, src, dst, _), directed in (("star5", shapes.star(5), False), ("sink4", shapes.sink_heavy(4), True)):
+    path = os.path.join(tmp, "shape.bin")
+    refdriver.write_graph(path, n, src, dst)
+    for app in ("pagerank", "pagerank_parallel"):
+        for mr in (0, 1):
+            arrays["%s_%s%d" % (name, app, mr)] = run(app, path, directed=directed, pr_d=0.85, mr=mr, threads=1)
+
 info = refdriver.run_rmat("bfs", 12, 16, 1, repeat=1)
 out["rmat12_seed1_bfs_info"] = {"source": int(info["source"]), "traversed_edges": int(info["traversed_edges"])}
 

@@ -82,6 +82,13 @@ def main():
         mm.close()
         return out, rounds, total
 
+    if os.environ.get("GL_SHAPES", "0") == "1":
+        run_shapes(pkg, gdist, pyoracle, rank, world, gather, failures)
+        flag = torch.tensor([len(failures)], device=dev)
+        dist.broadcast(flag, 0)
+        dist.destroy_process_group()
+        sys.exit(1 if int(flag.item()) else 0)
+
     for wmode, apps in ((0, ["bfs", "bfs_hub", "bfs_hub_src2", "bfs_hub_nodlg", "bfs_spill", "bfs_spill_src2", "bfs_nohub", "bfs_r1ship", "bfs_push", "bfs_step", "bfs_push_step", "wcc", "wcc_opt", "pagerank", "pagerank_pull", "cdlp", "lcc"]), (1, ["sssp", "face2_sssp"])):
         n = 1 << scale
         frag = pkg.Fragment.rmat(scale, 16, seed=17, weight_mode=wmode, fid=rank, fnum=world)
@@ -201,6 +208,53 @@ def main():
     dist.broadcast(flag, 0)
     dist.destroy_process_group()
     sys.exit(1 if int(flag.item()) else 0)
+
+
+def run_shapes(pkg, gdist, pyoracle, rank, world, gather, failures):
+    """GL_SHAPES=1: the constructed threshold graphs of tests/shapes.py split into
+    WORLD_SIZE fragments -- a star whose centre (fragment 0) has outer copies on
+    every peer, fragments without edges or outer vertices, owner boundaries inside
+    a bitmap word, a block of long rows and a long multi-edge -- through all six apps."""
+    from tests import shapes as S
+    cases = {"star": S.star(4097), "path": S.path(300), "path_then_isolated": S.pad_to(S.path(300), 1000),
+             "empty": S.empty(33), "hub_block": S.hub_block(33), "multi_loop": S.multi_loop()}
+    apps = [("bfs", dict(direction_opt=1)), ("bfs_push", dict(direction_opt=0)), ("bfs_step", dict(fuse_supersteps=0)),
+            ("sssp", {}), ("wcc", {}), ("wcc_opt", {}), ("pagerank", dict(pr_delta=0.85, max_round=10)),
+            ("pagerank_pull", dict(pr_delta=0.85, max_round=10, pr_pull=1)), ("cdlp", dict(max_round=5)), ("lcc", {})]
+    for shape, (n, src, dst, w) in cases.items():
+        frag = pkg.Fragment.from_edges(n, src, dst, w, fid=rank, fnum=world)
+        comm = gdist.make_comm(rank, world, frag.ivnum)
+        g = pyoracle.Graph(n, src, dst, w) if rank == 0 else None
+        source = 0                                   # the star centre, an end of the path, an isolated vertex
+        for name, cfg in apps:
+            kind = name.split("_")[0] if name != "wcc_opt" else name
+            if kind in ("bfs", "sssp"):
+                cfg = dict(cfg, source_oid=source)
+            app = pkg.App(kind, frag, comm, **cfg)
+            app.query()
+            got = gather(app.result())
+            if rank == 0:
+                if kind == "bfs":
+                    ok = np.array_equal(got, g.bfs(source)[0])
+                elif kind == "sssp":
+                    ok = np.array_equal(got, g.sssp(source)[0])
+                elif kind in ("wcc", "wcc_opt"):
+                    ok = np.array_equal(got, g.wcc()[0].astype(np.int64))
+                elif kind == "cdlp":
+                    ok = np.array_equal(got, g.cdlp(5))
+                elif kind == "lcc":
+                    ok = np.array_equal(got, g.lcc()[0])
+                else:
+                    want = g.pagerank(0.85, 10, 1)
+                    ok = bool(np.max(np.abs(got - want) / want) < 1e-6)
+                print("[mgpu] shape %-18s %-13s fnum=%d n=%d %s" % (shape, name, world, n, "OK" if ok else "MISMATCH"),
+                      flush=True)
+                if not ok:
+                    failures.append(shape + ":" + name)
+            app.close()
+            dist.barrier()
+        comm.close()
+        frag.close()
 
 
 if __name__ == "__main__":

@@ -55,3 +55,20 @@ def test_multi_fragment_one_device(nproc, scale, apps, min_ok):
     sys.stdout.write(p.stdout[-4000:])
     assert p.returncode == 0, p.stdout[-4000:]
     assert p.stdout.count(" OK") >= min_ok, p.stdout[-4000:]
+
+
+@pytest.mark.parametrize("nproc", [2, 3])
+def test_multi_fragment_shapes_one_device(nproc):
+    """The threshold graphs of tests/shapes.py (star, path, empty, hub block, multi-edge) split into
+    fragments on one device: fragments without edges or outer vertices, owner boundaries inside a
+    bitmap word, a hub with outer copies on every peer -- all six apps (mgpu_worker.py GL_SHAPES=1)."""
+    if _ngpus() < 1:
+        pytest.skip("needs a GPU")
+    env = dict(os.environ, GL_ONE_DEVICE="1", GL_SHAPES="1")
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", str(nproc),
+           "--master-addr", "127.0.0.1", "--master-port", str(29540 + nproc),
+           os.path.join(ROOT, "tests", "mgpu_worker.py")]
+    p = subprocess.run(cmd, cwd=ROOT, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=900)
+    sys.stdout.write(p.stdout[-4000:])
+    assert p.returncode == 0, p.stdout[-4000:]
+    assert p.stdout.count(" OK") == 60, p.stdout[-4000:]     # 6 shapes x 10 app configurations
