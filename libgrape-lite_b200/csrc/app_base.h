@@ -19,9 +19,9 @@ struct Engine {
   cudaStream_t stream = nullptr;
   int sm_count = 0;
   int grid = 0;            // persistent grid: SMs x resident CTAs
-  ScanCtrl* ctrl = nullptr;    // device
-  ScanCtrl* h_ctrl = nullptr;  // pinned host mirror
-  HubItem* hubs = nullptr;
+  DevBuf<ScanCtrl> ctrl;
+  PinnedBuf<ScanCtrl> h_ctrl;  // host mirror
+  DevBuf<HubItem> hubs;
   uint32_t hub_cap = 0;
   uint32_t hub_deg = kHubDeg;
   int init(const gl_frag* f);
@@ -83,12 +83,12 @@ struct gl_app {
 
 namespace gl {
 // hub-first (descending degree) order of the inner vertices: perm[lid] = rank, order[rank] = lid
-int build_hub_order(cudaStream_t s, const uint64_t* rp, uint32_t n, uint32_t** perm_out, uint32_t** order_out);
+int build_hub_order(cudaStream_t s, const uint64_t* rp, uint32_t n, DevBuf<uint32_t>* perm_out, DevBuf<uint32_t>* order_out);
 int build_permuted_csr(cudaStream_t s, const uint64_t* rp, const uint32_t* col, uint64_t m, uint32_t n,
-                       const uint32_t* order, const uint32_t* perm, uint64_t** rp_out, uint32_t** col_out,
-                       const void* w4 = nullptr, void** w4_out = nullptr, bool sort_rows = true);
+                       const uint32_t* order, const uint32_t* perm, DevBuf<uint64_t>* rp_out, DevBuf<uint32_t>* col_out,
+                       const void* w4 = nullptr, DevBuf<uint32_t>* w4_out = nullptr, bool sort_rows = true);
 // every row [rp[i], rp[i+1]) of *col sorted ascending (the array is replaced by a sorted copy)
-int sort_csr_rows(cudaStream_t s, const uint64_t* rp, uint32_t n, uint64_t m, uint32_t** col);
+int sort_csr_rows(cudaStream_t s, const uint64_t* rp, uint32_t n, uint64_t m, DevBuf<uint32_t>* col);
 gl_app* make_bfs();
 gl_app* make_sssp_f32();
 gl_app* make_sssp_f64();

@@ -1517,8 +1517,8 @@ __global__ void k_depth_u8_from_levels(const uint32_t* lv, uint32_t words, uint3
 }
 
 struct BfsApp : gl_app {
-  uint32_t *lv = nullptr, *vis = nullptr, *remote = nullptr, *hub_nbr = nullptr;
-  int64_t* out64 = nullptr;
+  DevBuf<uint32_t> lv, vis, remote, hub_nbr;
+  DevBuf<int64_t> out64;
   // the adjacency BFS runs on: the fragment's own CSR, or (single fragment) a
   // hub-first relabelled shadow copy — see hub_order.cu
   const uint64_t* g_rp = nullptr;
@@ -1527,23 +1527,23 @@ struct BfsApp : gl_app {
   // adjacency the pull step scans (== g_* unless the fragment is directed)
   const uint64_t* p_rp = nullptr;
   const uint32_t* p_col = nullptr;
-  uint32_t* nz_in = nullptr;   // directed: inner vertices with in-degree > 0
+  DevBuf<uint32_t> nz_in;   // directed: inner vertices with in-degree > 0
   // several fragments, fused kernel: gid-space copies for the replicated global frontier
-  uint32_t *gcol = nullptr, *hub_nbr_g = nullptr;
-  uint32_t* dlg_list = nullptr;   // delegated hubs: my inner neighbours of hub h = dlg_list[dlg_off[h] .. dlg_off[h + 1])
-  uint64_t* dlg_off = nullptr;
-  uint32_t* ovgid_p = nullptr;   // hub-first order over several fragments: the outer copies' gids in the owners' new lid space
+  DevBuf<uint32_t> gcol, hub_nbr_g;
+  DevBuf<uint32_t> dlg_list;   // delegated hubs: my inner neighbours of hub h = dlg_list[dlg_off[h] .. dlg_off[h + 1])
+  DevBuf<uint64_t> dlg_off;
+  DevBuf<uint32_t> ovgid_p;   // hub-first order over several fragments: the outer copies' gids in the owners' new lid space
   bool hub_multi = false;
   uint32_t seg_words = 0, seg_stride = 0, seg_gens = 1;
   bool global_front = false;
-  uint32_t *perm = nullptr, *order = nullptr, *nz_p = nullptr, *col_p = nullptr;
-  uint64_t* rp_p = nullptr;
+  DevBuf<uint32_t> perm, order, nz_p, col_p;
+  DevBuf<uint64_t> rp_p;
   // one fragment in hub-first order: rows of two or more entries are lids [0, multi_v); the fused
   // kernel's tail candidate list (kTailList entries)
   static constexpr uint32_t kTailList = 1u << 16;
   static constexpr uint32_t kListTry = 16;   // the list is tried from kListTry x kTailList unvisited vertices on
   uint32_t multi_v = 0;
-  uint32_t* tail_list = nullptr;
+  DevBuf<uint32_t> tail_list;
   uint32_t src_ = 0;
   int has_src_ = 0;
   unsigned long long nz_total = 0, visited_cnt = 0;
@@ -1556,35 +1556,12 @@ struct BfsApp : gl_app {
   uint64_t n_f = 0, m_f = 0, visited_edges = 0;
   uint64_t g_m_total = 0, g_vnum = 0, g_nz_total = 0;   // whole-graph totals (all fragments)
   uint32_t phase = 0;
-  BfsFusedCtl* d_ctl = nullptr;
-  BfsFusedCtl* h_ctl = nullptr;
+  DevBuf<BfsFusedCtl> d_ctl;
+  PinnedBuf<BfsFusedCtl> h_ctl;
   int fused_grid = 0;
 
   ~BfsApp() override {
-    cudaFree(d_ctl);
-    if (h_ctl) cudaFreeHost(h_ctl);
-    cudaFree(lv);
-    cudaFree(vis);
-    cudaFree(remote);
-    cudaFree(hub_nbr);
-    cudaFree(out64);
-    cudaFree(perm);
-    cudaFree(order);
-    cudaFree(spill);
-    cudaFree(nz_p);
-    cudaFree(col_p);
-    cudaFree(rp_p);
-    cudaFree(tail_list);
-    cudaFree(nz_in);
-    cudaFree(gcol);
-    cudaFree(hub_nbr_g);
-    cudaFree(ovgid_p);
-    cudaFree(dlg_list);
-    cudaFree(dlg_off);
-    cudaFree(d_out8);
-    cudaFree(deg8);
     if (ev_done) cudaEventDestroy(ev_done);
-    if (h_out8) cudaFreeHost(h_out8);
     for (auto e : ev8)
       if (e) cudaEventDestroy(e);
   }
@@ -1601,6 +1578,21 @@ struct BfsApp : gl_app {
   // can only push; levels are identical either way.
   bool can_pull() const { return cfg.direction_opt && (!fv.directed || !frag->ie_alias_oe); }
 
+  // Hub-first shadow graph (hub_order.cu): BFS runs on a copy of the adjacency with the inner vertices
+  // relabelled by descending degree, and the source moves to its new lid.
+  int BuildHubFirst() {
+    GL_TRY(build_hub_order(eng.stream, fv.oe_rp, fv.ivnum, &perm, &order));
+    GL_TRY(build_permuted_csr(eng.stream, fv.oe_rp, fv.oe_col, frag->oe.entries, fv.ivnum, order, perm, &rp_p, &col_p));
+    GL_CUDA(nz_p.alloc(words));
+    GL_CUDA(cudaMemsetAsync(nz_p, 0, sizeof(uint32_t) * words, eng.stream));
+    if (fv.ivnum) GL_LAUNCH(k_bfs_nz, (fv.ivnum + 255) / 256, 256, eng.stream, rp_p, fv.ivnum, nz_p);
+    g_rp = rp_p;
+    g_col = col_p;
+    g_nz = nz_p;
+    if (has_src_) GL_CUDA(cudaMemcpy(&src_, perm + src_, 4, cudaMemcpyDeviceToHost));
+    return GL_OK;
+  }
+
   int Setup() override {
     tvnum = fv.ivnum + fv.ovnum;
     words = (bm_words(tvnum) + 4) & ~(size_t) 3;
@@ -1608,32 +1600,26 @@ struct BfsApp : gl_app {
     size_t budget = (size_t) 1 << 30;
     max_lv = (uint32_t) std::max<size_t>(16, std::min<size_t>(4096, budget / (words * 4)));
     if (cfg.reserved[3] >= 4) max_lv = (uint32_t) cfg.reserved[3];   // test hook: tiny ring => spills
-    GL_CUDA(cudaMalloc(&lv, sizeof(uint32_t) * words * max_lv));
+    GL_CUDA(lv.alloc(words * max_lv));
     GL_CUDA(cudaMemsetAsync(lv, 0, sizeof(uint32_t) * words * max_lv, eng.stream));
-    GL_CUDA(cudaMalloc(&vis, sizeof(uint32_t) * words));
-    GL_CUDA(cudaMalloc(&remote, sizeof(uint32_t) * words));
-    GL_CUDA(cudaMalloc(&hub_nbr, sizeof(uint32_t) * ((size_t) fv.ivnum + kSuperV)));
+    GL_CUDA(vis.alloc(words));
+    GL_CUDA(remote.alloc(words));
+    GL_CUDA(hub_nbr.alloc((size_t) fv.ivnum + kSuperV));
     GL_CUDA(cudaMemsetAsync(hub_nbr, 0xFF, sizeof(uint32_t) * ((size_t) fv.ivnum + kSuperV), eng.stream));
-    GL_CUDA(cudaMalloc(&out64, sizeof(int64_t) * std::max<uint32_t>(fv.ivnum, 1)));
-    GL_CUDA(cudaMalloc(&d_ctl, sizeof(BfsFusedCtl)));
-    GL_CUDA(cudaMallocHost(&h_ctl, sizeof(BfsFusedCtl)));
+    GL_CUDA(out64.alloc(std::max<uint32_t>(fv.ivnum, 1)));
+    GL_CUDA(d_ctl.alloc(1));
+    GL_CUDA(h_ctl.alloc(1));
     memset(h_ctl, 0, sizeof(BfsFusedCtl));
     g_rp = fv.oe_rp;
     g_col = fv.oe_col;
     g_nz = frag->nonzero_deg;
+    // the source is fixed per app (AppConfig): resolve it once
+    has_src_ = gl_frag_oid2lid(frag, cfg.source_oid, &src_) == GL_OK ? 1 : 0;
     // hub-first shadow graph (one fragment, undirected, large enough to matter)
-    if (fv.fnum == 1 && can_pull() && !fv.directed && ((fv.ivnum >= (1u << 16) && cfg.reserved[1] == 0) || cfg.reserved[1] == 2)) {
-      GL_TRY(build_hub_order(eng.stream, fv.oe_rp, fv.ivnum, &perm, &order));
-      GL_TRY(build_permuted_csr(eng.stream, fv.oe_rp, fv.oe_col, frag->oe.entries, fv.ivnum, order, perm, &rp_p, &col_p));
-      GL_CUDA(cudaMalloc(&nz_p, sizeof(uint32_t) * words));
-      GL_CUDA(cudaMemsetAsync(nz_p, 0, sizeof(uint32_t) * words, eng.stream));
-      GL_LAUNCH(k_bfs_nz, (fv.ivnum + 255) / 256, 256, eng.stream, rp_p, fv.ivnum, nz_p);
-      g_rp = rp_p;
-      g_col = col_p;
-      g_nz = nz_p;
-    }
+    if (fv.fnum == 1 && can_pull() && !fv.directed && ((fv.ivnum >= (1u << 16) && cfg.reserved[1] == 0) || cfg.reserved[1] == 2))
+      GL_TRY(BuildHubFirst());
     if (fv.ivnum && cfg.direction_opt) {
-      GL_CUDA(cudaMalloc(&deg8, fv.ivnum));
+      GL_CUDA(deg8.alloc(fv.ivnum));
       GL_LAUNCH(k_bfs_deg8, (fv.ivnum + 255) / 256, 256, eng.stream, g_rp, fv.ivnum, deg8);
     }
     p_rp = g_rp;
@@ -1641,7 +1627,7 @@ struct BfsApp : gl_app {
     if (fv.directed && can_pull()) {
       p_rp = fv.ie_rp;
       p_col = fv.ie_col;
-      GL_CUDA(cudaMalloc(&nz_in, sizeof(uint32_t) * words));
+      GL_CUDA(nz_in.alloc(words));
       GL_CUDA(cudaMemsetAsync(nz_in, 0, sizeof(uint32_t) * words, eng.stream));
       if (fv.ivnum) GL_LAUNCH(k_bfs_nz, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, fv.ivnum, nz_in);
       g_nz = nz_in;   // pull candidates / "still reachable" statistics: in-degree > 0
@@ -1653,8 +1639,8 @@ struct BfsApp : gl_app {
       else GL_LAUNCH(k_bfs_hub_nbr, eng.sm_count * 8, 256, eng.stream, p_rp, row_end(), p_col, fv.ivnum, hub_nbr);
     }
     {
-      unsigned long long* d_cnt = nullptr;
-      GL_CUDA(cudaMalloc(&d_cnt, 16));
+      DevBuf<unsigned long long> d_cnt;
+      GL_CUDA(d_cnt.alloc(2));
       GL_CUDA(cudaMemsetAsync(d_cnt, 0, 16, eng.stream));
       GL_LAUNCH(k_bfs_popc, eng.sm_count * 4, 256, eng.stream, g_nz, (uint32_t) bm_words(fv.ivnum), d_cnt);
       GL_CUDA(cudaMemcpyAsync(&nz_total, d_cnt, 8, cudaMemcpyDeviceToHost, eng.stream));
@@ -1665,14 +1651,10 @@ struct BfsApp : gl_app {
         GL_CUDA(cudaMemcpyAsync(&m2, d_cnt + 1, 8, cudaMemcpyDeviceToHost, eng.stream));
         GL_CUDA(cudaStreamSynchronize(eng.stream));
         multi_v = (uint32_t) m2;
-        GL_CUDA(cudaMalloc(&tail_list, sizeof(uint32_t) * kTailList));
+        GL_CUDA(tail_list.alloc(kTailList));
       }
       GL_CUDA(cudaStreamSynchronize(eng.stream));
-      cudaFree(d_cnt);
     }
-    // the source is fixed per app (AppConfig): resolve it once
-    has_src_ = gl_frag_oid2lid(frag, cfg.source_oid, &src_) == GL_OK ? 1 : 0;
-    if (has_src_ && perm) GL_CUDA(cudaMemcpy(&src_, perm + src_, 4, cudaMemcpyDeviceToHost));
     GL_CUDA(cudaStreamSynchronize(eng.stream));
     used_lv = 0;
     // message = bare lid (bfs.h:50-51: sizeof(vid_t) per outer vertex)
@@ -1715,28 +1697,22 @@ struct BfsApp : gl_app {
                   ((cfg.reserved[1] == 0 && g_vnum >= (1u << 16)) || cfg.reserved[1] == 2 || cfg.reserved[1] == 3);
       if (hub_multi) {
         const uint64_t m = frag->oe.entries;
-        GL_TRY(build_hub_order(eng.stream, fv.oe_rp, fv.ivnum, &perm, &order));
-        GL_TRY(build_permuted_csr(eng.stream, fv.oe_rp, fv.oe_col, m, fv.ivnum, order, perm, &rp_p, &col_p));
-        GL_CUDA(cudaMalloc(&nz_p, sizeof(uint32_t) * words));
-        GL_CUDA(cudaMemsetAsync(nz_p, 0, sizeof(uint32_t) * words, eng.stream));
-        if (fv.ivnum) GL_LAUNCH(k_bfs_nz, (fv.ivnum + 255) / 256, 256, eng.stream, rp_p, fv.ivnum, nz_p);
-        g_rp = p_rp = rp_p;
-        g_col = p_col = col_p;
-        g_nz = nz_p;
+        GL_TRY(BuildHubFirst());
+        p_rp = g_rp;
+        p_col = g_col;
         if (deg8 && fv.ivnum) GL_LAUNCH(k_bfs_deg8, (fv.ivnum + 255) / 256, 256, eng.stream, g_rp, fv.ivnum, deg8);
-        if (has_src_) GL_CUDA(cudaMemcpy(&src_, perm + src_, 4, cudaMemcpyDeviceToHost));
         // owners' new lids reach the outer copies through one dense mirror sync
-        uint32_t* newlid = nullptr;
-        GL_CUDA(cudaMalloc(&newlid, sizeof(uint32_t) * std::max<size_t>(tvnum, 1)));
+        DevBuf<uint32_t> newlid;
+        GL_CUDA(newlid.alloc(std::max<size_t>(tvnum, 1)));
         GL_CUDA(cudaMemsetAsync(newlid, 0, sizeof(uint32_t) * std::max<size_t>(tvnum, 1), eng.stream));
         if (fv.ivnum) GL_CUDA(cudaMemcpyAsync(newlid, perm, sizeof(uint32_t) * fv.ivnum, cudaMemcpyDeviceToDevice, eng.stream));
         GL_TRY(mm.SyncValuesToGhosts(eng.stream, newlid, 4));
-        GL_CUDA(cudaMalloc(&ovgid_p, sizeof(uint32_t) * std::max<uint32_t>(fv.ovnum, 1)));
+        GL_CUDA(ovgid_p.alloc(std::max<uint32_t>(fv.ovnum, 1)));
         if (fv.ovnum)
           GL_LAUNCH(k_bfs_ovgid_new, (fv.ovnum + 255) / 256, 256, eng.stream, fv.ovgid, newlid + fv.ivnum, fv.ovnum, fv.id_mask, ovgid_p);
         const uint32_t gid0 = fv.fid << fv.fid_offset;
-        GL_CUDA(cudaMalloc(&gcol, sizeof(uint32_t) * (m + 16)));
-        GL_CUDA(cudaMalloc(&hub_nbr_g, sizeof(uint32_t) * ((size_t) fv.ivnum + kSuperV)));
+        GL_CUDA(gcol.alloc(m + 16));
+        GL_CUDA(hub_nbr_g.alloc((size_t) fv.ivnum + kSuperV));
         GL_CUDA(cudaMemsetAsync(hub_nbr_g, 0xFF, sizeof(uint32_t) * ((size_t) fv.ivnum + kSuperV), eng.stream));
         if (m) {
           GL_LAUNCH(k_bfs_gcol, eng.sm_count * 8, 256, eng.stream, p_col, m, fv.ivnum, gid0, ovgid_p, gcol);
@@ -1748,8 +1724,8 @@ struct BfsApp : gl_app {
         if (fv.ivnum) GL_LAUNCH(k_bfs_first_col, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, gcol, fv.ivnum, hub_nbr_g);
         if (cfg.reserved[1] != 3) {   // ([1] = 3: hub-first order without the delegated hubs, A/B)
           const uint32_t K = fv.fnum * kDlgPerFrag;
-          uint32_t* cnt = nullptr;
-          GL_CUDA(cudaMalloc(&cnt, sizeof(uint32_t) * K));
+          DevBuf<uint32_t> cnt;
+          GL_CUDA(cnt.alloc(K));
           GL_CUDA(cudaMemsetAsync(cnt, 0, sizeof(uint32_t) * K, eng.stream));
           if (fv.ivnum)
             GL_LAUNCH(k_bfs_dlg_scan, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, gcol, fv.ivnum, fv.fid_offset, fv.id_mask, cnt,
@@ -1759,37 +1735,34 @@ struct BfsApp : gl_app {
           GL_CUDA(cudaStreamSynchronize(eng.stream));
           std::vector<uint64_t> h_off(K + 1, 0);
           for (uint32_t h = 0; h < K; ++h) h_off[h + 1] = h_off[h] + h_cnt[h];
-          GL_CUDA(cudaMalloc(&dlg_off, sizeof(uint64_t) * (K + 1)));
+          GL_CUDA(dlg_off.alloc(K + 1));
           GL_CUDA(cudaMemcpyAsync(dlg_off, h_off.data(), sizeof(uint64_t) * (K + 1), cudaMemcpyHostToDevice, eng.stream));
-          GL_CUDA(cudaMalloc(&dlg_list, sizeof(uint32_t) * (h_off[K] + 16)));
+          GL_CUDA(dlg_list.alloc(h_off[K] + 16));
           GL_CUDA(cudaMemsetAsync(cnt, 0, sizeof(uint32_t) * K, eng.stream));
           if (fv.ivnum)
             GL_LAUNCH(k_bfs_dlg_scan, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, gcol, fv.ivnum, fv.fid_offset, fv.id_mask, cnt,
                       dlg_off, dlg_list, 1);
           GL_TRY(sort_csr_rows(eng.stream, dlg_off, K, h_off[K], &dlg_list));   // ascending lid: neighbouring bits, neighbouring words
           GL_CUDA(cudaStreamSynchronize(eng.stream));
-          cudaFree(cnt);
         }
         GL_CUDA(cudaStreamSynchronize(eng.stream));
-        cudaFree(newlid);
       } else if (can_pull() && fv.ivnum + fv.ovnum) {
         // the hub-neighbour prefilter should pick the true highest-degree neighbour, also when it is an
         // outer copy: owners' degrees reach the ghosts through one dense mirror sync (collective)
-        uint32_t* deg32 = nullptr;
-        GL_CUDA(cudaMalloc(&deg32, sizeof(uint32_t) * (size_t) tvnum));
+        DevBuf<uint32_t> deg32;
+        GL_CUDA(deg32.alloc(tvnum));
         GL_LAUNCH(k_bfs_deg32, (tvnum + 255) / 256, 256, eng.stream, fv.oe_rp, fv.ivnum, tvnum, deg32);
         GL_TRY(mm.SyncValuesToGhosts(eng.stream, deg32, 4));
         if (fv.ivnum) GL_LAUNCH(k_bfs_hub_nbr, eng.sm_count * 8, 256, eng.stream, p_rp, row_end(), p_col, fv.ivnum, hub_nbr, deg32);
         GL_CUDA(cudaStreamSynchronize(eng.stream));
-        cudaFree(deg32);
       } else if (can_pull()) {
         GL_TRY(mm.SyncValuesToGhosts(eng.stream, nullptr, 4));   // keep the collective sequence identical on every rank
       }
       if (global_front && !hub_multi) {
         const uint64_t m = (fv.directed ? frag->ie.entries : frag->oe.entries);
         const uint32_t gid0 = fv.fid << fv.fid_offset;
-        GL_CUDA(cudaMalloc(&gcol, sizeof(uint32_t) * (m + 16)));
-        GL_CUDA(cudaMalloc(&hub_nbr_g, sizeof(uint32_t) * ((size_t) fv.ivnum + kSuperV)));
+        GL_CUDA(gcol.alloc(m + 16));
+        GL_CUDA(hub_nbr_g.alloc((size_t) fv.ivnum + kSuperV));
         GL_CUDA(cudaMemsetAsync(hub_nbr_g, 0xFF, sizeof(uint32_t) * ((size_t) fv.ivnum + kSuperV), eng.stream));
         if (m) GL_LAUNCH(k_bfs_gcol, eng.sm_count * 8, 256, eng.stream, p_col, m, fv.ivnum, gid0, fv.ovgid, gcol);
         if (fv.ivnum) GL_LAUNCH(k_bfs_gid_table, (fv.ivnum + 255) / 256, 256, eng.stream, hub_nbr, fv.ivnum, fv.ivnum, gid0, fv.ovgid, hub_nbr_g);
@@ -1834,13 +1807,13 @@ struct BfsApp : gl_app {
   // frontier): move the depths of ring levels [0, max_lv-1) to the int32 side
   // array, restart the ring with the frontier at level 0.  BFS depth is then
   // only bounded by int32 like the reference's depth array (bfs.h:31).
-  int32_t* spill = nullptr;
+  DevBuf<int32_t> spill;
   bool spilled = false;
   uint32_t depth_base = 0;
   int SpillRing() {
     cudaStream_t s = eng.stream;
     if (!spill) {
-      GL_CUDA(cudaMalloc(&spill, sizeof(int32_t) * std::max<uint32_t>(fv.ivnum, 1)));
+      GL_CUDA(spill.alloc(std::max<uint32_t>(fv.ivnum, 1)));
       GL_CUDA(cudaMemsetAsync(spill, 0xFF, sizeof(int32_t) * std::max<uint32_t>(fv.ivnum, 1), s));
     }
     if (fv.ivnum)
@@ -1896,7 +1869,7 @@ struct BfsApp : gl_app {
     a.pa.sweep_v = hub_first ? (uint32_t) nz_total : fv.ivnum;
     a.pa.multi_v = hub_first ? multi_v : 0u;
     a.push_v = hub_first ? std::min<uint32_t>(fv.ivnum, std::max<uint32_t>((uint32_t) nz_total, src + 1)) : fv.ivnum;
-    a.pa.list = hub_first ? tail_list : nullptr;
+    a.pa.list = hub_first ? tail_list.get() : nullptr;
     a.pa.list_cap = hub_first ? kTailList : 0u;
     a.list_gap = kListTry * kTailList;
     if (!fused_grid)
@@ -2155,15 +2128,15 @@ struct BfsApp : gl_app {
   // the reference's int64 (bfs_context.h:31 depth_type) by host threads while the
   // next chunk is still crossing PCIe
   cudaEvent_t ev_done = nullptr;
-  uint8_t* deg8 = nullptr;
-  uint8_t *d_out8 = nullptr, *h_out8 = nullptr;
+  DevBuf<uint8_t> deg8, d_out8;
+  PinnedBuf<uint8_t> h_out8;
   cudaEvent_t ev8[8] = {};
   int ResultCompact(int64_t* host_out, uint32_t nl) {
     cudaStream_t s = eng.stream;
     const uint32_t n = fv.ivnum;
     if (!d_out8) {
-      GL_CUDA(cudaMalloc(&d_out8, n));
-      GL_CUDA(cudaMallocHost(&h_out8, n));
+      GL_CUDA(d_out8.alloc(n));
+      GL_CUDA(h_out8.alloc(n));
       for (auto& e : ev8) GL_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     }
     GL_LAUNCH(k_depth_u8_from_levels, (n + 255) / 256, 256, s, lv, (uint32_t) words, nl, n, perm, d_out8);
@@ -2202,7 +2175,7 @@ struct BfsApp : gl_app {
     if (compact_ok && !spilled && depth_base == 0 && nl <= 254 && cfg.reserved[6] == 0)
       return ResultCompact((int64_t*) host_out, nl);
     GL_LAUNCH(k_depth_from_levels, (fv.ivnum + 255) / 256, 256, eng.stream, lv, (uint32_t) words, nl, fv.ivnum, perm,
-              depth_base, spilled ? spill : nullptr, out64);
+              depth_base, spilled ? spill.get() : nullptr, out64);
     GL_CUDA(cudaMemcpyAsync(host_out, out64, sizeof(int64_t) * fv.ivnum, cudaMemcpyDeviceToHost, eng.stream));
     GL_CUDA(cudaStreamSynchronize(eng.stream));
     return GL_OK;

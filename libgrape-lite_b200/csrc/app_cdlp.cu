@@ -87,34 +87,26 @@ __global__ void k_cdlp_out(const uint32_t* label, uint32_t n, LabelMap lm, int64
 }
 
 struct CdlpApp : gl_app {
-  uint32_t *label = nullptr, *next = nullptr, *scratch = nullptr, *sorted = nullptr;
-  int64_t* out64 = nullptr;
-  void* sort_tmp = nullptr;
+  DevBuf<uint32_t> label, next, scratch, sorted;
+  DevBuf<int64_t> out64;
+  DevBuf<char> sort_tmp;
   size_t sort_bytes = 0;
   uint32_t tvnum = 0;
   int step = 0;
 
-  ~CdlpApp() override {
-    cudaFree(label);
-    cudaFree(next);
-    cudaFree(scratch);
-    cudaFree(sorted);
-    cudaFree(out64);
-    cudaFree(sort_tmp);
-  }
   size_t ResultElemBytes() const override { return sizeof(int64_t); }
 
   int Setup() override {
     tvnum = fv.ivnum + fv.ovnum;
     const uint64_t m = frag->oe.entries;
-    GL_CUDA(cudaMalloc(&label, sizeof(uint32_t) * std::max<uint32_t>(tvnum, 1)));
-    GL_CUDA(cudaMalloc(&next, sizeof(uint32_t) * std::max<uint32_t>(tvnum, 1)));
-    GL_CUDA(cudaMalloc(&scratch, sizeof(uint32_t) * std::max<uint64_t>(m, 4)));
-    GL_CUDA(cudaMalloc(&sorted, sizeof(uint32_t) * std::max<uint64_t>(m, 4)));
-    GL_CUDA(cudaMalloc(&out64, sizeof(int64_t) * std::max<uint32_t>(fv.ivnum, 1)));
-    GL_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, sort_bytes, scratch, sorted, (int64_t) m,
+    GL_CUDA(label.alloc(std::max<uint32_t>(tvnum, 1)));
+    GL_CUDA(next.alloc(std::max<uint32_t>(tvnum, 1)));
+    GL_CUDA(scratch.alloc(std::max<uint64_t>(m, 4)));
+    GL_CUDA(sorted.alloc(std::max<uint64_t>(m, 4)));
+    GL_CUDA(out64.alloc(std::max<uint32_t>(fv.ivnum, 1)));
+    GL_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, sort_bytes, scratch.get(), sorted.get(), (int64_t) m,
                                                (int64_t) fv.ivnum, fv.oe_rp, fv.oe_rp + 1, eng.stream));
-    GL_CUDA(cudaMalloc(&sort_tmp, std::max<size_t>(sort_bytes, 16)));
+    GL_CUDA(sort_tmp.alloc(std::max<size_t>(sort_bytes, 16)));
     GL_TRY(mm.Init(comm, fv, sizeof(ItemU32U32)));
     // outer copies read their owner's label every round (dense mirror sync;
     // the reference ships changed labels with SendMsgThroughOEdges, cdlp.h:69-70)
@@ -133,7 +125,7 @@ struct CdlpApp : gl_app {
     if (fv.fnum > 1 && step > 1) GL_TRY(mm.SyncValuesToGhosts(s, label, 4));
     if (m) {
       GL_LAUNCH(k_cdlp_gather, eng.sm_count * 8, 256, s, fv.oe_col, m, label, scratch);
-      GL_CUDA(cub::DeviceSegmentedSort::SortKeys(sort_tmp, sort_bytes, scratch, sorted, (int64_t) m,
+      GL_CUDA(cub::DeviceSegmentedSort::SortKeys(sort_tmp, sort_bytes, scratch.get(), sorted.get(), (int64_t) m,
                                                  (int64_t) fv.ivnum, fv.oe_rp, fv.oe_rp + 1, s));
       g_kernel_launches += 3;  // cub's partition + large/small segment kernels
     }

@@ -259,59 +259,37 @@ __global__ void k_lcc_out(const uint64_t* rp, const unsigned long long* tri,
 }
 
 struct LccApp : gl_app {
-  uint64_t *cnt = nullptr, *orp = nullptr;
-  uint32_t *ocol = nullptr, *osrc = nullptr;   // fnum > 1: ocol holds gids (sorted per row)
-  uint32_t *olid = nullptr, *deg = nullptr, *remote = nullptr;
-  unsigned long long* tri = nullptr;
-  double* out64 = nullptr;
+  DevBuf<uint64_t> cnt, orp;
+  DevBuf<uint32_t> ocol, osrc;   // fnum > 1: ocol holds gids (sorted per row)
+  DevBuf<uint32_t> olid, deg, remote;
+  DevBuf<unsigned long long> tri;
+  DevBuf<double> out64;
   uint64_t om = 0;
   int stage = 0;
   uint32_t tvnum = 0;
   size_t words = 0;
-  // replicas of the peers' DAG parts (fnum > 1)
-  std::vector<uint64_t*> r_orp;
-  std::vector<uint32_t*> r_key;
-  const uint64_t** d_t_orp = nullptr;
-  const uint32_t** d_t_key = nullptr;
+  // replicas of the peers' DAG parts (fnum > 1; the entry of this fragment stays empty)
+  std::vector<DevBuf<uint64_t>> rep_orp;
+  std::vector<DevBuf<uint32_t>> rep_key;
+  // device tables [fnum] of the DAG parts: the replicas, and orp / ocol at [fid]
+  DevBuf<const uint64_t*> d_t_orp;
+  DevBuf<const uint32_t*> d_t_key;
 
-  void free_replicas() {
-    for (size_t g = 0; g < r_orp.size(); ++g) {
-      if (g == fv.fid) continue;
-      cudaFree(r_orp[g]);
-      cudaFree(r_key[g]);
-    }
-    r_orp.clear();
-    r_key.clear();
-  }
-  ~LccApp() override {
-    free_replicas();
-    cudaFree(cnt);
-    cudaFree(orp);
-    cudaFree(ocol);
-    cudaFree(osrc);
-    cudaFree(olid);
-    cudaFree(deg);
-    cudaFree(remote);
-    cudaFree(tri);
-    cudaFree(out64);
-    cudaFree(d_t_orp);
-    cudaFree(d_t_key);
-  }
   size_t ResultElemBytes() const override { return sizeof(double); }
 
   int Setup() override {
     tvnum = fv.ivnum + fv.ovnum;
     words = bm_words(tvnum) + 1;
-    GL_CUDA(cudaMalloc(&cnt, sizeof(uint64_t) * ((size_t) fv.ivnum + 1)));
-    GL_CUDA(cudaMalloc(&orp, sizeof(uint64_t) * ((size_t) fv.ivnum + 1)));
-    GL_CUDA(cudaMalloc(&tri, sizeof(unsigned long long) * std::max<uint32_t>(tvnum, 1)));
-    GL_CUDA(cudaMalloc(&out64, sizeof(double) * std::max<uint32_t>(fv.ivnum, 1)));
+    GL_CUDA(cnt.alloc((size_t) fv.ivnum + 1));
+    GL_CUDA(orp.alloc((size_t) fv.ivnum + 1));
+    GL_CUDA(tri.alloc(std::max<uint32_t>(tvnum, 1)));
+    GL_CUDA(out64.alloc(std::max<uint32_t>(fv.ivnum, 1)));
     GL_TRY(mm.Init(comm, fv, sizeof(ItemU32I64)));
     if (fv.fnum > 1) {
-      GL_CUDA(cudaMalloc(&deg, sizeof(uint32_t) * std::max<uint32_t>(tvnum, 1)));
-      GL_CUDA(cudaMalloc(&remote, sizeof(uint32_t) * words));
-      GL_CUDA(cudaMalloc(&d_t_orp, sizeof(void*) * fv.fnum));
-      GL_CUDA(cudaMalloc(&d_t_key, sizeof(void*) * fv.fnum));
+      GL_CUDA(deg.alloc(std::max<uint32_t>(tvnum, 1)));
+      GL_CUDA(remote.alloc(words));
+      GL_CUDA(d_t_orp.alloc(fv.fnum));
+      GL_CUDA(d_t_key.alloc(fv.fnum));
       GL_TRY(mm.BuildMirrorPlan(eng.stream, fv));
     }
     return GL_OK;
@@ -327,29 +305,23 @@ struct LccApp : gl_app {
   int scan_counts(uint64_t* total) {
     cudaStream_t s = eng.stream;
     size_t tb = 0;
-    GL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, orp, (int) (fv.ivnum + 1), s));
-    void* tmp = nullptr;
-    GL_CUDA(cudaMalloc(&tmp, std::max<size_t>(tb, 16)));
-    cudaError_t e = cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, orp, (int) (fv.ivnum + 1), s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(total, orp + fv.ivnum, 8, cudaMemcpyDeviceToHost, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    cudaFree(tmp);
-    if (e != cudaSuccess) {
-      set_error("LCC scan: %s", cudaGetErrorString(e));
-      return GL_ERR_CUDA;
-    }
+    GL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt.get(), orp.get(), (int) (fv.ivnum + 1), s));
+    DevBuf<char> tmp;
+    GL_CUDA(tmp.alloc(std::max<size_t>(tb, 16)));
+    GL_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, cnt.get(), orp.get(), (int) (fv.ivnum + 1), s));
+    GL_CUDA(cudaMemcpyAsync(total, orp + fv.ivnum, 8, cudaMemcpyDeviceToHost, s));
+    GL_CUDA(cudaStreamSynchronize(s));
     return GL_OK;
   }
   int resize_dag(uint64_t total) {
     if (total != om || !ocol) {
-      cudaFree(ocol);
-      cudaFree(osrc);
-      cudaFree(olid);
-      ocol = osrc = olid = nullptr;
+      ocol.reset();
+      osrc.reset();
+      olid.reset();
       om = total;
-      GL_CUDA(cudaMalloc(&ocol, sizeof(uint32_t) * std::max<uint64_t>(om, 4)));
-      GL_CUDA(cudaMalloc(&osrc, sizeof(uint32_t) * std::max<uint64_t>(om, 4)));
-      if (fv.fnum > 1) GL_CUDA(cudaMalloc(&olid, sizeof(uint32_t) * std::max<uint64_t>(om, 4)));
+      GL_CUDA(ocol.alloc(std::max<uint64_t>(om, 4)));
+      GL_CUDA(osrc.alloc(std::max<uint64_t>(om, 4)));
+      if (fv.fnum > 1) GL_CUDA(olid.alloc(std::max<uint64_t>(om, 4)));
     }
     return GL_OK;
   }
@@ -379,21 +351,18 @@ struct LccApp : gl_app {
     GL_TRY(scan_counts(&total));
     GL_TRY(resize_dag(total));
     if (fv.ivnum && om) {
-      uint32_t *key_u = nullptr, *lid_u = nullptr;
-      GL_CUDA(cudaMalloc(&key_u, sizeof(uint32_t) * om));
-      GL_CUDA(cudaMalloc(&lid_u, sizeof(uint32_t) * om));
+      DevBuf<uint32_t> key_u, lid_u;
+      GL_CUDA(key_u.alloc(om));
+      GL_CUDA(lid_u.alloc(om));
       GL_LAUNCH(k_lcc_fill_m, eng.sm_count * 8, 256, s, fv.oe_rp, fv.oe_col, deg, gid, fv.ivnum, orp, key_u, lid_u, osrc);
       size_t sb = 0;
-      GL_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, sb, key_u, ocol, lid_u, olid, (int64_t) om,
-                                                  (int64_t) fv.ivnum, orp, orp + 1, s));
-      void* st = nullptr;
-      GL_CUDA(cudaMalloc(&st, std::max<size_t>(sb, 16)));
-      GL_CUDA(cub::DeviceSegmentedSort::SortPairs(st, sb, key_u, ocol, lid_u, olid, (int64_t) om,
-                                                  (int64_t) fv.ivnum, orp, orp + 1, s));
+      GL_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, sb, key_u.get(), ocol.get(), lid_u.get(), olid.get(), (int64_t) om,
+                                                  (int64_t) fv.ivnum, orp.get(), orp + 1, s));
+      DevBuf<char> st;
+      GL_CUDA(st.alloc(std::max<size_t>(sb, 16)));
+      GL_CUDA(cub::DeviceSegmentedSort::SortPairs(st, sb, key_u.get(), ocol.get(), lid_u.get(), olid.get(), (int64_t) om,
+                                                  (int64_t) fv.ivnum, orp.get(), orp + 1, s));
       GL_CUDA(cudaStreamSynchronize(s));
-      cudaFree(st);
-      cudaFree(key_u);
-      cudaFree(lid_u);
     }
     // 3. export my arrays, replicate the peers' (bulk NVLink copies)
     LccExport mine;
@@ -404,9 +373,12 @@ struct LccApp : gl_app {
     mine.om = om;
     std::vector<char> all;
     GL_TRY(mm.ExchangeBlobs(s, &mine, sizeof(mine), &all));
-    free_replicas();
-    r_orp.assign(fv.fnum, nullptr);
-    r_key.assign(fv.fnum, nullptr);
+    rep_orp.clear();
+    rep_key.clear();
+    rep_orp.resize(fv.fnum);
+    rep_key.resize(fv.fnum);
+    std::vector<const uint64_t*> r_orp(fv.fnum);
+    std::vector<const uint32_t*> r_key(fv.fnum);
     for (uint32_t g = 0; g < fv.fnum; ++g) {
       if (g == fv.fid) {
         r_orp[g] = orp;
@@ -414,13 +386,15 @@ struct LccApp : gl_app {
         continue;
       }
       const LccExport& ex = *(const LccExport*) (all.data() + (size_t) g * sizeof(LccExport));
-      GL_CUDA(cudaMalloc(&r_orp[g], sizeof(uint64_t) * (ex.ivnum + 1)));
-      GL_CUDA(cudaMalloc(&r_key[g], sizeof(uint32_t) * std::max<uint64_t>(ex.om, 4)));
+      GL_CUDA(rep_orp[g].alloc(ex.ivnum + 1));
+      GL_CUDA(rep_key[g].alloc(std::max<uint64_t>(ex.om, 4)));
+      r_orp[g] = rep_orp[g];
+      r_key[g] = rep_key[g];
       void *p_orp = nullptr, *p_key = nullptr;
       GL_CUDA(cudaIpcOpenMemHandle(&p_orp, ex.h_orp, cudaIpcMemLazyEnablePeerAccess));
       GL_CUDA(cudaIpcOpenMemHandle(&p_key, ex.h_key, cudaIpcMemLazyEnablePeerAccess));
-      GL_CUDA(cudaMemcpyAsync(r_orp[g], p_orp, sizeof(uint64_t) * (ex.ivnum + 1), cudaMemcpyDeviceToDevice, s));
-      if (ex.om) GL_CUDA(cudaMemcpyAsync(r_key[g], p_key, sizeof(uint32_t) * ex.om, cudaMemcpyDeviceToDevice, s));
+      GL_CUDA(cudaMemcpyAsync(rep_orp[g], p_orp, sizeof(uint64_t) * (ex.ivnum + 1), cudaMemcpyDeviceToDevice, s));
+      if (ex.om) GL_CUDA(cudaMemcpyAsync(rep_key[g], p_key, sizeof(uint32_t) * ex.om, cudaMemcpyDeviceToDevice, s));
       GL_CUDA(cudaStreamSynchronize(s));
       GL_CUDA(cudaIpcCloseMemHandle(p_orp));
       GL_CUDA(cudaIpcCloseMemHandle(p_key));

@@ -102,19 +102,6 @@ __global__ void k_pr_contrib(const double* rank, const uint64_t* rp,
     contrib[perm ? perm[i] : i] = (CT) (dg ? rank[i] / (double) dg : 0.0);
   }
 }
-__global__ void k_pr_degkey(const uint64_t* rp, uint32_t n, uint32_t* key, uint32_t* val) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) {
-    uint64_t dg = rp[i + 1] - rp[i];
-    if (dg > 0xFFFFFFFFull) dg = 0xFFFFFFFFull;
-    key[i] = 0xFFFFFFFFu - (uint32_t) dg;   // ascending key = descending degree
-    val[i] = i;
-  }
-}
-__global__ void k_pr_invert(const uint32_t* order, uint32_t n, uint32_t* perm) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) perm[order[i]] = i;
-}
 __global__ void k_pr_permute_cols(const uint32_t* __restrict__ col, uint64_t m,
                                   const uint32_t* __restrict__ perm, uint32_t n, uint32_t* out) {
   for (uint64_t i = (uint64_t) blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (uint64_t) gridDim.x * blockDim.x) {
@@ -291,9 +278,9 @@ __global__ void k_ones(uint32_t* bm, uint32_t nbits, uint32_t words) {
 }
 
 struct PageRankApp : gl_app {
-  double *rank = nullptr, *next = nullptr, *contrib = nullptr, *d_dangling = nullptr;
-  uint32_t* all_inner = nullptr;
-  uint32_t *perm = nullptr, *col_p = nullptr;   // hub-first gather order (pull, one fragment)
+  DevBuf<double> rank, next, contrib, d_dangling;
+  DevBuf<uint32_t> all_inner;
+  DevBuf<uint32_t> perm, col_p;   // hub-first gather order (pull, one fragment): perm[u] = rank of u by descending degree; col_p = perm[col]
   size_t words = 0;
   uint32_t tvnum = 0;
   int curr_iter = 0;
@@ -303,61 +290,28 @@ struct PageRankApp : gl_app {
   // push formulation (same ranks, pagerank.h:207-221), never a wrong gather.
   bool use_pull() const { return cfg.pr_pull && !fv.directed; }
 
-  ~PageRankApp() override {
-    cudaFree(rank);
-    cudaFree(next);
-    cudaFree(contrib);
-    cudaFree(d_dangling);
-    cudaFree(all_inner);
-    cudaFree(perm);
-    cudaFree(col_p);
-  }
   size_t ResultElemBytes() const override { return sizeof(double); }
 
   int Setup() override {
     tvnum = fv.ivnum + fv.ovnum;
     words = bm_words(fv.ivnum) + 1;
-    GL_CUDA(cudaMalloc(&rank, sizeof(double) * std::max<uint32_t>(tvnum, 1)));
-    GL_CUDA(cudaMalloc(&next, sizeof(double) * std::max<uint32_t>(tvnum, 1)));
-    GL_CUDA(cudaMalloc(&d_dangling, sizeof(double)));
-    GL_CUDA(cudaMalloc(&all_inner, sizeof(uint32_t) * words));
+    GL_CUDA(rank.alloc(std::max<uint32_t>(tvnum, 1)));
+    GL_CUDA(next.alloc(std::max<uint32_t>(tvnum, 1)));
+    GL_CUDA(d_dangling.alloc(1));
+    GL_CUDA(all_inner.alloc(words));
     GL_LAUNCH(k_ones, (unsigned) ((words + 255) / 256), 256, eng.stream, all_inner, fv.ivnum, (uint32_t) words);
     if (use_pull()) {
-      GL_CUDA(cudaMalloc(&contrib, sizeof(double) * std::max<uint32_t>(tvnum, 1)));
-      if (fv.fnum == 1 && fv.ivnum) GL_TRY(BuildHubOrder());
+      GL_CUDA(contrib.alloc(std::max<uint32_t>(tvnum, 1)));
+      if (fv.fnum == 1 && fv.ivnum) {
+        const uint64_t m = frag->oe.entries;
+        GL_TRY(build_hub_order(eng.stream, fv.oe_rp, fv.ivnum, &perm, nullptr));
+        GL_CUDA(col_p.alloc(m + 16));
+        if (m) GL_LAUNCH(k_pr_permute_cols, eng.sm_count * 8, 256, eng.stream, fv.oe_col, m, perm, fv.ivnum, col_p);
+        GL_CUDA(cudaStreamSynchronize(eng.stream));
+      }
     }
     GL_TRY(mm.Init(comm, fv, sizeof(ItemU32F64)));
     if (use_pull() && fv.fnum > 1) GL_TRY(mm.BuildMirrorPlan(eng.stream, fv));
-    return GL_OK;
-  }
-
-  // perm[u] = rank of u by descending degree; col_p = perm[col]
-  int BuildHubOrder() {
-    cudaStream_t s = eng.stream;
-    const uint32_t n = fv.ivnum;
-    const uint64_t m = frag->oe.entries;
-    uint32_t *key = nullptr, *key2 = nullptr, *val = nullptr, *val2 = nullptr;
-    GL_CUDA(cudaMalloc(&key, 4ull * n));
-    GL_CUDA(cudaMalloc(&key2, 4ull * n));
-    GL_CUDA(cudaMalloc(&val, 4ull * n));
-    GL_CUDA(cudaMalloc(&val2, 4ull * n));
-    GL_LAUNCH(k_pr_degkey, (n + 255) / 256, 256, s, fv.oe_rp, n, key, val);
-    size_t tb = 0;
-    cub::DoubleBuffer<uint32_t> kb(key, key2), vb(val, val2);
-    GL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, kb, vb, (int) n, 0, 32, s));
-    void* tmp = nullptr;
-    GL_CUDA(cudaMalloc(&tmp, std::max<size_t>(tb, 16)));
-    GL_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, kb, vb, (int) n, 0, 32, s));
-    GL_CUDA(cudaMalloc(&perm, 4ull * n));
-    GL_LAUNCH(k_pr_invert, (n + 255) / 256, 256, s, vb.Current(), n, perm);
-    GL_CUDA(cudaMalloc(&col_p, 4ull * (m + 16)));
-    if (m) GL_LAUNCH(k_pr_permute_cols, eng.sm_count * 8, 256, s, fv.oe_col, m, perm, n, col_p);
-    GL_CUDA(cudaStreamSynchronize(s));
-    cudaFree(key);
-    cudaFree(key2);
-    cudaFree(val);
-    cudaFree(val2);
-    cudaFree(tmp);
     return GL_OK;
   }
 
@@ -376,7 +330,7 @@ struct PageRankApp : gl_app {
   // contributions -> (mirror sync) -> next = base + delta * gathered sums
   template <typename CT>
   int pull_sweep(cudaStream_t s, double base) {
-    CT* cb = (CT*) contrib;
+    CT* cb = (CT*) contrib.get();
     l2_persist_window(s, cb, sizeof(CT) * (size_t) tvnum);   // the gathered array stays in L2, the CSR streams through
     if (fv.ivnum) GL_LAUNCH(k_pr_contrib<CT>, (fv.ivnum + 255) / 256, 256, s, rank, fv.oe_rp, fv.ivnum, perm, cb);
     // outer copies take their owner's contribution (dense mirror sync)

@@ -137,42 +137,34 @@ __global__ void k_dist_to_f64(const T* d, uint32_t n, T inf, double* out) {
 
 template <typename T>
 struct SsspApp : gl_app {
-  T* dist = nullptr;
-  uint32_t *in_q = nullptr, *near = nullptr, *far = nullptr, *remote = nullptr;
-  double* out64 = nullptr;
+  DevBuf<T> dist;
+  DevBuf<uint32_t> in_q, near, far, remote;
+  DevBuf<double> out64;
   size_t words = 0;
   uint32_t tvnum = 0;
   T init_prio = 0, prio = 0;
   uint64_t far_total = 0;
   static T inf() { return sizeof(T) == 4 ? (T) FLT_MAX : (T) DBL_MAX; }
 
-  ~SsspApp() override {
-    cudaFree(dist);
-    cudaFree(in_q);
-    cudaFree(near);
-    cudaFree(far);
-    cudaFree(remote);
-    cudaFree(out64);
-  }
   size_t ResultElemBytes() const override { return sizeof(double); }
 
   int Setup() override {
     tvnum = fv.ivnum + fv.ovnum;
     words = bm_words(tvnum) + 1;
-    GL_CUDA(cudaMalloc(&dist, sizeof(T) * std::max<uint32_t>(tvnum, 1)));
-    GL_CUDA(cudaMalloc(&in_q, sizeof(uint32_t) * words));
-    GL_CUDA(cudaMalloc(&near, sizeof(uint32_t) * words));
-    GL_CUDA(cudaMalloc(&far, sizeof(uint32_t) * words));
-    GL_CUDA(cudaMalloc(&remote, sizeof(uint32_t) * words));
-    GL_CUDA(cudaMalloc(&out64, sizeof(double) * std::max<uint32_t>(fv.ivnum, 1)));
+    GL_CUDA(dist.alloc(std::max<uint32_t>(tvnum, 1)));
+    GL_CUDA(in_q.alloc(words));
+    GL_CUDA(near.alloc(words));
+    GL_CUDA(far.alloc(words));
+    GL_CUDA(remote.alloc(words));
+    GL_CUDA(out64.alloc(std::max<uint32_t>(fv.ivnum, 1)));
     // init_prio heuristic (sssp.h:76-92)
     double p = cfg.sssp_prio;
     {
       double wsum = (double) frag->oe.entries;  // unweighted: every edge counts 1
       if (frag->oe.w && frag->oe.entries) {
-        double* d_sum;
         double h_sum[2] = {0, 0};
-        GL_CUDA(cudaMalloc(&d_sum, 16));
+        DevBuf<double> d_sum;
+        GL_CUDA(d_sum.alloc(2));
         GL_CUDA(cudaMemsetAsync(d_sum, 0, 16, eng.stream));
         if (fv.edata_bytes == 4) {
           GL_LAUNCH(k_weight_sum<float>, eng.sm_count * 8, 256, eng.stream, (const float*) frag->oe.w, frag->oe.entries, d_sum);
@@ -181,7 +173,7 @@ struct SsspApp : gl_app {
         }
         GL_CUDA(cudaMemcpyAsync(h_sum, d_sum, 16, cudaMemcpyDeviceToHost, eng.stream));
         GL_CUDA(cudaStreamSynchronize(eng.stream));
-        cudaFree(d_sum);
+        d_sum.reset();
         wsum = h_sum[0];
         if (h_sum[1] != 0.0) {
           set_error("SSSP: negative (or -0.0 / NaN) edge weights are not supported");

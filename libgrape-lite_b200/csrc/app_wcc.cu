@@ -103,19 +103,12 @@ __global__ void k_wcc_out(const uint32_t* label, uint32_t n, LabelMap lm, int64_
 }
 
 struct WccApp : gl_app {
-  uint32_t *label = nullptr, *in_q = nullptr, *out_local = nullptr, *remote = nullptr;
-  int64_t* out64 = nullptr;
+  DevBuf<uint32_t> label, in_q, out_local, remote;
+  DevBuf<int64_t> out64;
   size_t words = 0;
   uint32_t tvnum = 0;
   uint64_t active_estimate = 0;   // vertices active in the coming round
 
-  ~WccApp() override {
-    cudaFree(label);
-    cudaFree(in_q);
-    cudaFree(out_local);
-    cudaFree(remote);
-    cudaFree(out64);
-  }
   size_t ResultElemBytes() const override { return sizeof(int64_t); }
 
   int Setup() override {
@@ -127,11 +120,11 @@ struct WccApp : gl_app {
     }
     tvnum = fv.ivnum + fv.ovnum;
     words = bm_words(tvnum) + 1;
-    GL_CUDA(cudaMalloc(&label, sizeof(uint32_t) * std::max<uint32_t>(tvnum, 1)));
-    GL_CUDA(cudaMalloc(&in_q, sizeof(uint32_t) * words));
-    GL_CUDA(cudaMalloc(&out_local, sizeof(uint32_t) * words));
-    GL_CUDA(cudaMalloc(&remote, sizeof(uint32_t) * words));
-    GL_CUDA(cudaMalloc(&out64, sizeof(int64_t) * std::max<uint32_t>(fv.ivnum, 1)));
+    GL_CUDA(label.alloc(std::max<uint32_t>(tvnum, 1)));
+    GL_CUDA(in_q.alloc(words));
+    GL_CUDA(out_local.alloc(words));
+    GL_CUDA(remote.alloc(words));
+    GL_CUDA(out64.alloc(std::max<uint32_t>(fv.ivnum, 1)));
     return mm.Init(comm, fv, sizeof(ItemU32U32));
   }
 

@@ -225,21 +225,12 @@ __global__ void k_uf_out(const uint32_t* par, const uint32_t* clabel, uint32_t n
 }
 
 struct WccOptApp : gl_app {
-  uint32_t *par = nullptr, *clabel = nullptr, *sent = nullptr, *rest = nullptr, *remote = nullptr, *d_giant = nullptr;
-  int64_t* out64 = nullptr;
+  DevBuf<uint32_t> par, clabel, sent, rest, remote, d_giant;
+  DevBuf<int64_t> out64;
   uint32_t tvnum = 0;
   size_t words = 0;
   static constexpr uint32_t kSampled = 2;
 
-  ~WccOptApp() override {
-    cudaFree(par);
-    cudaFree(clabel);
-    cudaFree(sent);
-    cudaFree(rest);
-    cudaFree(remote);
-    cudaFree(d_giant);
-    cudaFree(out64);
-  }
   size_t ResultElemBytes() const override { return sizeof(int64_t); }
 
   int Setup() override {
@@ -251,13 +242,13 @@ struct WccOptApp : gl_app {
     }
     tvnum = fv.ivnum + fv.ovnum;
     words = bm_words(tvnum) + 1;
-    GL_CUDA(cudaMalloc(&par, sizeof(uint32_t) * std::max<uint32_t>(tvnum, 1)));
-    GL_CUDA(cudaMalloc(&clabel, sizeof(uint32_t) * std::max<uint32_t>(tvnum, 1)));
-    GL_CUDA(cudaMalloc(&sent, sizeof(uint32_t) * std::max<uint32_t>(fv.ovnum, 1)));
-    GL_CUDA(cudaMalloc(&rest, sizeof(uint32_t) * words));
-    GL_CUDA(cudaMalloc(&remote, sizeof(uint32_t) * words));
-    GL_CUDA(cudaMalloc(&d_giant, sizeof(uint32_t)));
-    GL_CUDA(cudaMalloc(&out64, sizeof(int64_t) * std::max<uint32_t>(fv.ivnum, 1)));
+    GL_CUDA(par.alloc(std::max<uint32_t>(tvnum, 1)));
+    GL_CUDA(clabel.alloc(std::max<uint32_t>(tvnum, 1)));
+    GL_CUDA(sent.alloc(std::max<uint32_t>(fv.ovnum, 1)));
+    GL_CUDA(rest.alloc(words));
+    GL_CUDA(remote.alloc(words));
+    GL_CUDA(d_giant.alloc(1));
+    GL_CUDA(out64.alloc(std::max<uint32_t>(fv.ivnum, 1)));
     return mm.Init(comm, fv, sizeof(ItemU32U32));
   }
 

@@ -249,7 +249,7 @@ int MessageManager::PeerBarrierAsync(cudaStream_t s) {
   const unsigned long long tag = ++comm->seq_base;
   const int par = (int) (tag & 1);
   const PeerSlot* local = (const PeerSlot*) (comm->local_base + GL_COMM_SLOT_OFF) + (size_t) par * GL_MAX_FNUM;
-  if (!d_scratch_result) GL_CUDA(cudaMalloc(&d_scratch_result, sizeof(PeerSlot)));
+  if (!d_scratch_result) GL_CUDA(d_scratch_result.alloc(1));
   GL_LAUNCH(k_peer_allreduce, 1, GL_MAX_FNUM, s, fnum, fid, d_peer_slot[par], local, tag, 0ll, 0ll, 0.0, 0,
             nullptr, nullptr, nullptr, d_scratch_result, 0ll, 0ll, nullptr, nullptr);
   return GL_OK;
@@ -304,8 +304,8 @@ int MessageManager::BuildMirrorPlan(cudaStream_t s, const gl_frag_view& fv) {
       snd[p] = comm->peer_base[p] + comm->mirror_off(par, fid);
       rcv[p] = comm->local_base + comm->mirror_off(par, p);
     }
-    GL_CUDA(cudaMalloc(&d_msend[par], sizeof(char*) * fnum));
-    GL_CUDA(cudaMalloc(&d_mrecv[par], sizeof(char*) * fnum));
+    GL_CUDA(d_msend[par].alloc(fnum));
+    GL_CUDA(d_mrecv[par].alloc(fnum));
     GL_CUDA(cudaMemcpy(d_msend[par], snd.data(), sizeof(char*) * fnum, cudaMemcpyHostToDevice));
     GL_CUDA(cudaMemcpy(d_mrecv[par], rcv.data(), sizeof(char*) * fnum, cudaMemcpyHostToDevice));
   }
@@ -334,8 +334,8 @@ int MessageManager::BuildMirrorPlan(cudaStream_t s, const gl_frag_view& fv) {
   mirror_off.assign(fnum + 1, 0);
   for (uint32_t g = 0; g < fnum; ++g) mirror_off[g + 1] = mirror_off[g] + (g == fid ? 0 : cnt[g]);
   mirror_total = mirror_off[fnum];
-  GL_CUDA(cudaMalloc(&d_mirror_lids, sizeof(uint32_t) * std::max<uint64_t>(mirror_total, 1)));
-  GL_CUDA(cudaMalloc(&d_mirror_off, sizeof(uint64_t) * (fnum + 1)));
+  GL_CUDA(d_mirror_lids.alloc(std::max<uint64_t>(mirror_total, 1)));
+  GL_CUDA(d_mirror_off.alloc(fnum + 1));
   GL_CUDA(cudaMemcpy(d_mirror_off, mirror_off.data(), sizeof(uint64_t) * (fnum + 1), cudaMemcpyHostToDevice));
   for (uint32_t g = 0; g < fnum; ++g) {
     if (g == fid || cnt[g] == 0) continue;
@@ -349,24 +349,25 @@ int MessageManager::BuildMirrorPlan(cudaStream_t s, const gl_frag_view& fv) {
   // word-parallel form for bit syncs (needs ascending lids per holder)
   mirror_sorted = false;
   if (mirror_total && fv.ivnum) {
-    uint32_t* d_bad = nullptr;
-    GL_CUDA(cudaMalloc(&d_bad, 4));
-    GL_CUDA(cudaMemsetAsync(d_bad, 0, 4, s));
     dim3 grid(num_sms() * 4, fnum);
-    k_mirror_check_sorted<<<grid, 256, 0, s>>>(d_mirror_lids, d_mirror_off, fnum, d_bad);
     uint32_t bad = 1;
-    GL_CUDA(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
-    GL_CUDA(cudaStreamSynchronize(s));
-    cudaFree(d_bad);
+    {
+      DevBuf<uint32_t> d_bad;
+      GL_CUDA(d_bad.alloc(1));
+      GL_CUDA(cudaMemsetAsync(d_bad, 0, 4, s));
+      k_mirror_check_sorted<<<grid, 256, 0, s>>>(d_mirror_lids, d_mirror_off, fnum, d_bad);
+      GL_CUDA(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, s));
+      GL_CUDA(cudaStreamSynchronize(s));
+    }
     if (!bad) {
       iv_words = (uint32_t) ((fv.ivnum + 31) / 32);
       std::vector<uint64_t> woff(fnum + 1, 0);
       for (uint32_t g = 0; g < fnum; ++g) woff[g + 1] = woff[g] + (mirror_off[g + 1] - mirror_off[g] + 31) / 32;
       mirror_out_words = woff[fnum];
-      GL_CUDA(cudaMalloc(&d_mirror_mask, sizeof(uint32_t) * (size_t) fnum * iv_words));
-      GL_CUDA(cudaMalloc(&d_mirror_pref, sizeof(uint32_t) * (size_t) fnum * iv_words));
-      GL_CUDA(cudaMalloc(&d_mirror_startw, sizeof(uint32_t) * std::max<uint64_t>(mirror_out_words, 1)));
-      GL_CUDA(cudaMalloc(&d_mirror_woff, sizeof(uint64_t) * (fnum + 1)));
+      GL_CUDA(d_mirror_mask.alloc((size_t) fnum * iv_words));
+      GL_CUDA(d_mirror_pref.alloc((size_t) fnum * iv_words));
+      GL_CUDA(d_mirror_startw.alloc(std::max<uint64_t>(mirror_out_words, 1)));
+      GL_CUDA(d_mirror_woff.alloc(fnum + 1));
       GL_CUDA(cudaMemcpyAsync(d_mirror_woff, woff.data(), sizeof(uint64_t) * (fnum + 1), cudaMemcpyHostToDevice, s));
       GL_CUDA(cudaMemsetAsync(d_mirror_mask, 0, sizeof(uint32_t) * (size_t) fnum * iv_words, s));
       k_mirror_mask<<<grid, 256, 0, s>>>(d_mirror_lids, d_mirror_off, iv_words, d_mirror_mask);
@@ -463,10 +464,10 @@ int MessageManager::Init(gl_comm* c, const gl_frag_view& fv, uint32_t item_bytes
     set_error("fragment has fnum=%u but no opened communicator was supplied", fnum);
     return GL_ERR_COMM;
   }
-  GL_CUDA(cudaMalloc(&d_send_count, sizeof(uint32_t) * fnum));
+  GL_CUDA(d_send_count.alloc(fnum));
   GL_CUDA(cudaMemset(d_send_count, 0, sizeof(uint32_t) * fnum));
-  GL_CUDA(cudaMallocHost(&h_send_count, sizeof(uint32_t) * (fnum + 1)));
-  GL_CUDA(cudaMallocHost(&h_result, sizeof(PeerSlot)));
+  GL_CUDA(h_send_count.alloc(fnum + 1));
+  GL_CUDA(h_result.alloc(1));
   for (int par = 0; par < 2; ++par) {
     std::vector<char*> send(fnum);
     std::vector<const char*> recv(fnum);
@@ -483,53 +484,16 @@ int MessageManager::Init(gl_comm* c, const gl_frag_view& fv, uint32_t item_bytes
     std::vector<PeerSlot*> ps(fnum);
     for (uint32_t p = 0; p < fnum; ++p)
       ps[p] = (PeerSlot*) (c->peer_base[p] + GL_COMM_SLOT_OFF) + (size_t) par * GL_MAX_FNUM + fid;
-    GL_CUDA(cudaMalloc(&d_peer_slot[par], sizeof(PeerSlot*) * fnum));
+    GL_CUDA(d_peer_slot[par].alloc(fnum));
     GL_CUDA(cudaMemcpy(d_peer_slot[par], ps.data(), sizeof(PeerSlot*) * fnum, cudaMemcpyHostToDevice));
-    GL_CUDA(cudaMalloc(&d_send_slot[par], sizeof(char*) * fnum));
-    GL_CUDA(cudaMalloc(&d_recv_slot[par], sizeof(char*) * fnum));
-    GL_CUDA(cudaMalloc(&d_peer_count[par], sizeof(uint32_t*) * fnum));
+    GL_CUDA(d_send_slot[par].alloc(fnum));
+    GL_CUDA(d_recv_slot[par].alloc(fnum));
+    GL_CUDA(d_peer_count[par].alloc(fnum));
     GL_CUDA(cudaMemcpy(d_send_slot[par], send.data(), sizeof(char*) * fnum, cudaMemcpyHostToDevice));
     GL_CUDA(cudaMemcpy(d_recv_slot[par], recv.data(), sizeof(char*) * fnum, cudaMemcpyHostToDevice));
     GL_CUDA(cudaMemcpy(d_peer_count[par], pc.data(), sizeof(uint32_t*) * fnum, cudaMemcpyHostToDevice));
   }
   return GL_OK;
-}
-
-void MessageManager::Destroy() {
-  for (int par = 0; par < 2; ++par) {
-    if (d_send_slot[par]) cudaFree(d_send_slot[par]);
-    if (d_recv_slot[par]) cudaFree((void*) d_recv_slot[par]);
-    if (d_peer_count[par]) cudaFree(d_peer_count[par]);
-    if (d_peer_slot[par]) cudaFree(d_peer_slot[par]);
-    d_peer_slot[par] = nullptr;
-    d_send_slot[par] = nullptr;
-    d_recv_slot[par] = nullptr;
-    d_peer_count[par] = nullptr;
-  }
-  for (int par = 0; par < 2; ++par) {
-    if (d_msend[par]) cudaFree(d_msend[par]);
-    if (d_mrecv[par]) cudaFree((void*) d_mrecv[par]);
-    d_msend[par] = nullptr;
-    d_mrecv[par] = nullptr;
-  }
-  if (d_mirror_lids) cudaFree(d_mirror_lids);
-  if (d_mirror_off) cudaFree(d_mirror_off);
-  cudaFree(d_mirror_mask);
-  cudaFree(d_mirror_pref);
-  cudaFree(d_mirror_startw);
-  cudaFree(d_mirror_woff);
-  d_mirror_mask = d_mirror_pref = d_mirror_startw = nullptr;
-  d_mirror_woff = nullptr;
-  if (d_scratch_result) cudaFree(d_scratch_result);
-  d_scratch_result = nullptr;
-  d_mirror_lids = nullptr;
-  d_mirror_off = nullptr;
-  if (d_send_count) cudaFree(d_send_count);
-  if (h_send_count) cudaFreeHost(h_send_count);
-  if (h_result) cudaFreeHost(h_result);
-  h_result = nullptr;
-  d_send_count = nullptr;
-  h_send_count = nullptr;
 }
 
 MsgView MessageManager::view() const {
@@ -760,8 +724,8 @@ extern "C" int gl_comm_peer_write_us(gl_comm_t* c, size_t bytes, int vec16, int 
     set_error("gl_comm_peer_write_us: bytes must be in (0, mirror_bytes]");
     return GL_ERR_ARG;
   }
-  void* src = nullptr;
-  GL_CUDA(cudaMalloc(&src, bytes));
+  DevBuf<char> src;
+  GL_CUDA(src.alloc(bytes));
   GL_CUDA(cudaMemset(src, 1, bytes));
   std::vector<char*> dsts;
   for (uint32_t k = 1; k < c->fnum; ++k) {
@@ -769,16 +733,16 @@ extern "C" int gl_comm_peer_write_us(gl_comm_t* c, size_t bytes, int vec16, int 
     dsts.push_back(c->peer_base[p] + c->mirror_off(1, c->fid));   // my parity-1 mirror slot at peer p
     if (!all_peers) break;
   }
-  char** d_dsts = nullptr;
-  GL_CUDA(cudaMalloc(&d_dsts, sizeof(char*) * dsts.size()));
+  DevBuf<char*> d_dsts;
+  GL_CUDA(d_dsts.alloc(dsts.size()));
   GL_CUDA(cudaMemcpy(d_dsts, dsts.data(), sizeof(char*) * dsts.size(), cudaMemcpyHostToDevice));
   cudaEvent_t e0, e1;
   GL_CUDA(cudaEventCreate(&e0));
   GL_CUDA(cudaEventCreate(&e1));
   for (int r = -2; r < reps; ++r) {
     if (r == 0) GL_CUDA(cudaEventRecord(e0, 0));
-    if (vec16) k_peer_write<uint4><<<num_sms() * 4, 256>>>((const uint4*) src, (uint4* const*) d_dsts, (uint32_t) dsts.size(), bytes / 16);
-    else k_peer_write<uint32_t><<<num_sms() * 4, 256>>>((const uint32_t*) src, (uint32_t* const*) d_dsts, (uint32_t) dsts.size(), bytes / 4);
+    if (vec16) k_peer_write<uint4><<<num_sms() * 4, 256>>>((const uint4*) src.get(), (uint4* const*) d_dsts.get(), (uint32_t) dsts.size(), bytes / 16);
+    else k_peer_write<uint32_t><<<num_sms() * 4, 256>>>((const uint32_t*) src.get(), (uint32_t* const*) d_dsts.get(), (uint32_t) dsts.size(), bytes / 4);
   }
   GL_CUDA(cudaEventRecord(e1, 0));
   GL_CUDA(cudaEventSynchronize(e1));
@@ -787,8 +751,6 @@ extern "C" int gl_comm_peer_write_us(gl_comm_t* c, size_t bytes, int vec16, int 
   *us_out = (double) ms * 1e3 / reps;
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
-  cudaFree(d_dsts);
-  cudaFree(src);
   return GL_OK;
 }
 
@@ -802,7 +764,7 @@ struct gl_mm {
   gl::MessageManager mm;
   gl_comm* comm = nullptr;
   bool owns_single = false;   // fnum == 1 and no communicator was given
-  gl::ScanCtrl* d_ctrl = nullptr;
+  gl::DevBuf<gl::ScanCtrl> d_ctrl;
 };
 
 namespace gl {
@@ -949,14 +911,13 @@ int gl_bitmap_clear(void* stream, uint32_t* bitmap, uint64_t nbits) {
 int gl_bitmap_count(void* stream, const uint32_t* bitmap, uint64_t nbits, uint64_t* count_host) {
   GL_ARG(bitmap && count_host, "null argument");
   cudaStream_t s = (cudaStream_t) stream;
-  unsigned long long* d = nullptr;
-  GL_CUDA(cudaMalloc(&d, 8));
+  DevBuf<unsigned long long> d;
+  GL_CUDA(d.alloc(1));
   GL_CUDA(cudaMemsetAsync(d, 0, 8, s));
   if (nbits) GL_LAUNCH(k_bitmap_count, num_sms() * 4, 256, s, bitmap, nbits, d);
   unsigned long long h = 0;
   GL_CUDA(cudaMemcpyAsync(&h, d, 8, cudaMemcpyDeviceToHost, s));
   GL_CUDA(cudaStreamSynchronize(s));
-  cudaFree(d);
   *count_host = h;
   return GL_OK;
 }
@@ -1001,8 +962,7 @@ int gl_mm_create(gl_mm_t** out, gl_comm_t* comm) {
     delete m;
     return st;
   }
-  if (cudaMalloc(&m->d_ctrl, sizeof(ScanCtrl)) != cudaSuccess) {
-    m->mm.Destroy();
+  if (m->d_ctrl.alloc(1) != cudaSuccess) {
     delete m;
     set_error("gl_mm_create: device allocation failed");
     return GL_ERR_NOMEM;
@@ -1063,9 +1023,6 @@ int gl_mm_view_get(gl_mm_t* m, gl_mm_view* out) {
 }
 uint64_t gl_mm_bytes_sent(gl_mm_t* m) { return m ? m->mm.bytes_sent : 0; }
 void gl_mm_destroy(gl_mm_t* m) {
-  if (!m) return;
-  m->mm.Destroy();
-  if (m->d_ctrl) cudaFree(m->d_ctrl);
   delete m;
 }
 
@@ -1077,7 +1034,7 @@ int gl_mm_process(gl_mm_t* m, void* stream, const gl_msg_op* op, uint64_t* items
   cudaStream_t s = (cudaStream_t) stream;
   gl_mm_view mv;
   GL_TRY(gl_mm_view_get(m, &mv));
-  unsigned long long* cnt = (unsigned long long*) m->d_ctrl;
+  unsigned long long* cnt = (unsigned long long*) m->d_ctrl.get();
   GL_CUDA(cudaMemsetAsync(cnt, 0, 8, s));
   const int grid = num_sms() * 4;
   switch (op->kind) {

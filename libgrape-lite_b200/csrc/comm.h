@@ -97,14 +97,13 @@ struct MessageManager {
   bool terminate = false;
   uint64_t bytes_sent = 0;
   // device tables
-  char** d_send_slot[2] = {nullptr, nullptr};        // [parity][fnum]
-  const char** d_recv_slot[2] = {nullptr, nullptr};  // [parity][fnum]
-  uint32_t* d_send_count = nullptr;                  // [fnum]
-  uint32_t* h_send_count = nullptr;                  // pinned [fnum+1]
-  uint32_t** d_peer_count[2] = {nullptr, nullptr};   // [parity][fnum] address of my count cell at peer
+  DevBuf<char*> d_send_slot[2];          // [parity][fnum]
+  DevBuf<const char*> d_recv_slot[2];    // [parity][fnum]
+  DevBuf<uint32_t> d_send_count;         // [fnum]
+  PinnedBuf<uint32_t> h_send_count;      // [fnum+1]
+  DevBuf<uint32_t*> d_peer_count[2];     // [parity][fnum] address of my count cell at peer
 
   int Init(gl_comm* c, const gl_frag_view& fv, uint32_t item_bytes_);
-  void Destroy();
   // GPUMessageManager::StartARound / FinishARound / ToTerminate / ForceContinue
   void Start() { round = 0; force_continue = false; terminate = false; bytes_sent = 0; }
   int StartARound(cudaStream_t s);
@@ -135,7 +134,7 @@ struct MessageManager {
   // so a round closes with ONE host synchronisation.
   const ScanCtrl* vote_ctrl = nullptr;
   ScanCtrl* vote_h_ctrl = nullptr;
-  PeerSlot* d_scratch_result = nullptr;
+  DevBuf<PeerSlot> d_scratch_result;
   // ---- dense mirror sync (owner's inner state -> the outer copies held by
   // other fragments); replaces BatchShuffleMessageManager::SyncInnerVertices.
   // BuildMirrorPlan is collective and must run once (Setup); afterwards every
@@ -146,22 +145,22 @@ struct MessageManager {
   int SyncValuesToGhosts(cudaStream_t s, void* values, int elem_bytes);  // values[ghost] = owner value
   bool plan_built = false;
   uint32_t plan_ivnum = 0;
-  uint32_t* d_mirror_lids = nullptr;        // my inner lids mirrored elsewhere, grouped by holder
-  uint64_t* d_mirror_off = nullptr;         // device [fnum+1]
+  DevBuf<uint32_t> d_mirror_lids;          // my inner lids mirrored elsewhere, grouped by holder
+  DevBuf<uint64_t> d_mirror_off;            // device [fnum+1]
   std::vector<uint64_t> mirror_off;         // host  [fnum+1]
   uint64_t mirror_total = 0;
   uint32_t* d_ghost_range = nullptr;        // device [fnum+1]: outer lids owned by each fid (outer_range)
   std::vector<uint32_t> ghost_range;
-  char** d_msend[2] = {nullptr, nullptr};        // [parity][fnum] mirror slot (parity, me) at peer
-  const char** d_mrecv[2] = {nullptr, nullptr};  // [parity][fnum] my mirror slot (parity, src)
+  DevBuf<char*> d_msend[2];         // [parity][fnum] mirror slot (parity, me) at peer
+  DevBuf<const char*> d_mrecv[2];   // [parity][fnum] my mirror slot (parity, src)
   unsigned long long mirror_seq = 0;
   // word-parallel form of the plan for bit syncs (see MirrorBitsPlan below)
   bool mirror_sorted = false;
   uint32_t iv_words = 0;
-  uint32_t* d_mirror_mask = nullptr;     // [fnum][iv_words]
-  uint32_t* d_mirror_pref = nullptr;     // [fnum][iv_words]
-  uint32_t* d_mirror_startw = nullptr;   // [woff[fnum]]
-  uint64_t* d_mirror_woff = nullptr;     // [fnum+1] output words per holder (prefix)
+  DevBuf<uint32_t> d_mirror_mask;     // [fnum][iv_words]
+  DevBuf<uint32_t> d_mirror_pref;     // [fnum][iv_words]
+  DevBuf<uint32_t> d_mirror_startw;   // [woff[fnum]]
+  DevBuf<uint64_t> d_mirror_woff;     // [fnum+1] output words per holder (prefix)
   uint64_t mirror_out_words = 0;
   struct MirrorBitsPlan bits_plan() const;
   // extra statistics carried by the round vote (summed over fragments)
@@ -174,8 +173,8 @@ struct MessageManager {
   bool decided_terminate = false;
   cudaStream_t stream_for_collectives = nullptr;
   unsigned long long seq = 0;
-  PeerSlot** d_peer_slot[2] = {nullptr, nullptr};  // [parity][fnum] my slot at peer p
-  PeerSlot* h_result = nullptr;                    // pinned
+  DevBuf<PeerSlot*> d_peer_slot[2];  // [parity][fnum] my slot at peer p
+  PinnedBuf<PeerSlot> h_result;
 };
 
 #ifdef __CUDACC__

@@ -41,6 +41,56 @@ const char* last_error();
     }                                                          \
   } while (0)
 
+// Owning buffer of T: device memory (cudaMalloc), or pinned host memory
+// (cudaMallocHost) when kPinned.  Move-only; freed on destruction, so a buffer
+// is released on every return path.  alloc(n) takes exactly n * sizeof(T)
+// bytes: pads stay with the caller, and the memory is plain cudaMalloc memory
+// (CUDA IPC handles, free-memory accounting).  Converts to T* so that launches
+// and copies take it like the raw pointer.
+template <typename T, bool kPinned = false>
+class Buf {
+ public:
+  Buf() = default;
+  Buf(const Buf&) = delete;
+  Buf& operator=(const Buf&) = delete;
+  Buf(Buf&& o) noexcept : p_(o.release()) {}
+  Buf& operator=(Buf&& o) noexcept {
+    reset(o.release());
+    return *this;
+  }
+  ~Buf() { reset(); }
+
+  cudaError_t alloc(size_t n) {
+    reset();
+    void* q = nullptr;
+    cudaError_t e = kPinned ? cudaMallocHost(&q, n * sizeof(T)) : cudaMalloc(&q, n * sizeof(T));
+    p_ = (T*) q;
+    return e;
+  }
+  T* get() const { return p_; }
+  operator T*() const { return p_; }
+  T* operator->() const { return p_; }
+  T* release() {
+    T* q = p_;
+    p_ = nullptr;
+    return q;
+  }
+  void reset(T* q = nullptr) {
+    if (p_) {
+      if (kPinned) cudaFreeHost(p_);
+      else cudaFree(p_);
+    }
+    p_ = q;
+  }
+
+ private:
+  T* p_ = nullptr;
+};
+template <typename T>
+using DevBuf = Buf<T, false>;
+template <typename T>
+using PinnedBuf = Buf<T, true>;
+
 // device properties (cached per process; one device per process/thread)
 struct DeviceInfo {
   int device = -1;

@@ -247,48 +247,37 @@ inline unsigned nblk(uint64_t n, unsigned t = 256) {
   return (unsigned) ((n + t - 1) / t);
 }
 
-struct DevBuf {
-  void* p = nullptr;
-  ~DevBuf() {
-    if (p) cudaFree(p);
-  }
-  template <typename T>
-  T* as() {
-    return (T*) p;
-  }
-  void* release() {
-    void* q = p;
-    p = nullptr;
-    return q;
-  }
-};
-#define GL_ALLOC(buf, bytes) GL_CUDA(cudaMalloc(&(buf).p, (bytes) ? (bytes) : 16))
+// The builder's buffers take at least 16 bytes, so that an empty one is still a valid pointer.
+template <typename T>
+cudaError_t alloc16(DevBuf<T>& b, size_t n) {
+  return b.alloc(n ? n : 16 / sizeof(T));
+}
 
 int sort_keys_u64(uint64_t*& keys, uint64_t*& alt, void*& vals, void*& vals_alt,
                   int vbytes, uint64_t m, int end_bit) {
   if (m == 0) return GL_OK;
   size_t tmp_bytes = 0;
-  DevBuf tmp;
+  DevBuf<char> tmp;
   if (vbytes == 0) {
     cub::DoubleBuffer<uint64_t> kb(keys, alt);
     GL_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, kb, (int64_t) m, 0, end_bit));
-    GL_ALLOC(tmp, tmp_bytes);
-    GL_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, tmp_bytes, kb, (int64_t) m, 0, end_bit));
+    GL_CUDA(alloc16(tmp, tmp_bytes));
+    GL_CUDA(cub::DeviceRadixSort::SortKeys(tmp.get(), tmp_bytes, kb, (int64_t) m, 0, end_bit));
     if (kb.Current() != keys) std::swap(keys, alt);
   } else if (vbytes == 4) {
     cub::DoubleBuffer<uint64_t> kb(keys, alt);
     cub::DoubleBuffer<uint32_t> vb((uint32_t*) vals, (uint32_t*) vals_alt);
     GL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, kb, vb, (int64_t) m, 0, end_bit));
-    GL_ALLOC(tmp, tmp_bytes);
-    GL_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, kb, vb, (int64_t) m, 0, end_bit));
+    GL_CUDA(alloc16(tmp, tmp_bytes));
+    GL_CUDA(cub::DeviceRadixSort::SortPairs(tmp.get(), tmp_bytes, kb, vb, (int64_t) m, 0, end_bit));
     if (kb.Current() != keys) std::swap(keys, alt);
     if ((void*) vb.Current() != vals) std::swap(vals, vals_alt);
   } else {
     cub::DoubleBuffer<uint64_t> kb(keys, alt);
     cub::DoubleBuffer<uint64_t> vb((uint64_t*) vals, (uint64_t*) vals_alt);
     GL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, kb, vb, (int64_t) m, 0, end_bit));
-    GL_ALLOC(tmp, tmp_bytes);
-    GL_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, kb, vb, (int64_t) m, 0, end_bit));
+    GL_CUDA(alloc16(tmp, tmp_bytes));
+    GL_CUDA(cub::DeviceRadixSort::SortPairs(tmp.get(), tmp_bytes, kb, vb, (int64_t) m, 0, end_bit));
     if (kb.Current() != keys) std::swap(keys, alt);
     if ((void*) vb.Current() != vals) std::swap(vals, vals_alt);
   }
@@ -329,17 +318,17 @@ struct RmatProducer : Producer {
 struct HostProducer : Producer {
   const gl_edges_desc* d;
   const int64_t* d_oids = nullptr;
-  DevBuf ts, td;
+  DevBuf<int64_t> ts, td;
   uint64_t total() const override { return d->n_edges; }
   int fill(uint64_t first, uint32_t count, uint32_t* s, uint32_t* dd,
            void* w) override {
-    if (!ts.p) {
-      GL_ALLOC(ts, sizeof(int64_t) * (size_t) (1u << 24));
-      GL_ALLOC(td, sizeof(int64_t) * (size_t) (1u << 24));
+    if (!ts) {
+      GL_CUDA(alloc16(ts, (size_t) (1u << 24)));
+      GL_CUDA(alloc16(td, (size_t) (1u << 24)));
     }
-    GL_CUDA(cudaMemcpy(ts.p, d->src + first, sizeof(int64_t) * count, cudaMemcpyHostToDevice));
-    GL_CUDA(cudaMemcpy(td.p, d->dst + first, sizeof(int64_t) * count, cudaMemcpyHostToDevice));
-    k_map_oids<<<nblk(count), 256>>>(ts.as<int64_t>(), td.as<int64_t>(), count,
+    GL_CUDA(cudaMemcpy(ts.get(), d->src + first, sizeof(int64_t) * count, cudaMemcpyHostToDevice));
+    GL_CUDA(cudaMemcpy(td.get(), d->dst + first, sizeof(int64_t) * count, cudaMemcpyHostToDevice));
+    k_map_oids<<<nblk(count), 256>>>(ts.get(), td.get(), count,
                                      d_oids, d->n_vertices, s, dd);
     GL_COUNT_LAUNCH();
     GL_CUDA(cudaGetLastError());
@@ -374,35 +363,36 @@ int build_from_producer(gl_frag* f, Producer& prod, uint64_t n, int directed,
   GL_ARG(p.chunk <= (uint64_t) f->id_mask + 1, "fragment too large for 32-bit gid");
 
   const uint64_t E = prod.total();
-  DevBuf bs, bd, bw, c_oe, c_ie, scan_tmp;
-  GL_ALLOC(bs, sizeof(uint32_t) * (size_t) CH);
-  GL_ALLOC(bd, sizeof(uint32_t) * (size_t) CH);
-  if (edata_bytes) GL_ALLOC(bw, (size_t) edata_bytes * CH);
-  GL_ALLOC(c_oe, sizeof(uint32_t) * (size_t) (CH + 1));
-  GL_ALLOC(c_ie, sizeof(uint32_t) * (size_t) (CH + 1));
+  DevBuf<uint32_t> bs, bd, c_oe, c_ie;
+  DevBuf<char> bw, scan_tmp;
+  GL_CUDA(alloc16(bs, (size_t) CH));
+  GL_CUDA(alloc16(bd, (size_t) CH));
+  if (edata_bytes) GL_CUDA(alloc16(bw, (size_t) edata_bytes * CH));
+  GL_CUDA(alloc16(c_oe, (size_t) (CH + 1)));
+  GL_CUDA(alloc16(c_ie, (size_t) (CH + 1)));
   size_t scan_bytes = 0;
-  GL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, c_oe.as<uint32_t>(),
-                                        c_oe.as<uint32_t>(), (int) (CH + 1)));
-  GL_ALLOC(scan_tmp, scan_bytes);
+  GL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, c_oe.get(),
+                                        c_oe.get(), (int) (CH + 1)));
+  GL_CUDA(alloc16(scan_tmp, scan_bytes));
 
   // pass 1: totals
   std::vector<uint64_t> base_oe, base_ie;
   uint64_t m_oe = 0, m_ie = 0;
   for (uint64_t first = 0; first < E; first += CH) {
     uint32_t cnt = (uint32_t) std::min<uint64_t>(CH, E - first);
-    GL_TRY(prod.fill(first, cnt, bs.as<uint32_t>(), bd.as<uint32_t>(), nullptr));
-    GL_CUDA(cudaMemsetAsync(c_oe.p, 0, sizeof(uint32_t) * (cnt + 1)));
-    GL_CUDA(cudaMemsetAsync(c_ie.p, 0, sizeof(uint32_t) * (cnt + 1)));
-    k_count<<<nblk(cnt), 256>>>(bs.as<uint32_t>(), bd.as<uint32_t>(), cnt, p,
-                                directed, c_oe.as<uint32_t>(), c_ie.as<uint32_t>());
+    GL_TRY(prod.fill(first, cnt, bs.get(), bd.get(), nullptr));
+    GL_CUDA(cudaMemsetAsync(c_oe.get(), 0, sizeof(uint32_t) * (cnt + 1)));
+    GL_CUDA(cudaMemsetAsync(c_ie.get(), 0, sizeof(uint32_t) * (cnt + 1)));
+    k_count<<<nblk(cnt), 256>>>(bs.get(), bd.get(), cnt, p,
+                                directed, c_oe.get(), c_ie.get());
     GL_COUNT_LAUNCH();
-    GL_CUDA(cub::DeviceScan::ExclusiveSum(scan_tmp.p, scan_bytes, c_oe.as<uint32_t>(),
-                                          c_oe.as<uint32_t>(), (int) (cnt + 1)));
-    GL_CUDA(cub::DeviceScan::ExclusiveSum(scan_tmp.p, scan_bytes, c_ie.as<uint32_t>(),
-                                          c_ie.as<uint32_t>(), (int) (cnt + 1)));
+    GL_CUDA(cub::DeviceScan::ExclusiveSum(scan_tmp.get(), scan_bytes, c_oe.get(),
+                                          c_oe.get(), (int) (cnt + 1)));
+    GL_CUDA(cub::DeviceScan::ExclusiveSum(scan_tmp.get(), scan_bytes, c_ie.get(),
+                                          c_ie.get(), (int) (cnt + 1)));
     uint32_t t_oe = 0, t_ie = 0;
-    GL_CUDA(cudaMemcpy(&t_oe, c_oe.as<uint32_t>() + cnt, 4, cudaMemcpyDeviceToHost));
-    GL_CUDA(cudaMemcpy(&t_ie, c_ie.as<uint32_t>() + cnt, 4, cudaMemcpyDeviceToHost));
+    GL_CUDA(cudaMemcpy(&t_oe, c_oe.get() + cnt, 4, cudaMemcpyDeviceToHost));
+    GL_CUDA(cudaMemcpy(&t_ie, c_ie.get() + cnt, 4, cudaMemcpyDeviceToHost));
     base_oe.push_back(m_oe);
     base_ie.push_back(m_ie);
     m_oe += t_oe;
@@ -410,133 +400,139 @@ int build_from_producer(gl_frag* f, Producer& prod, uint64_t n, int directed,
   }
 
   // pass 2: emit keys (+weights)
-  DevBuf k_oe, k_oe2, w_oe, w_oe2, k_ie, k_ie2, w_ie, w_ie2;
-  GL_ALLOC(k_oe, sizeof(uint64_t) * m_oe);
-  GL_ALLOC(k_oe2, sizeof(uint64_t) * m_oe);
+  DevBuf<uint64_t> k_oe, k_oe2, k_ie, k_ie2;
+  DevBuf<char> w_oe, w_oe2, w_ie, w_ie2;
+  GL_CUDA(alloc16(k_oe, m_oe));
+  GL_CUDA(alloc16(k_oe2, m_oe));
   if (edata_bytes) {
-    GL_ALLOC(w_oe, (size_t) edata_bytes * m_oe + 64);
-    GL_ALLOC(w_oe2, (size_t) edata_bytes * m_oe + 64);
+    GL_CUDA(alloc16(w_oe, (size_t) edata_bytes * m_oe + 64));
+    GL_CUDA(alloc16(w_oe2, (size_t) edata_bytes * m_oe + 64));
   }
   if (directed) {
-    GL_ALLOC(k_ie, sizeof(uint64_t) * m_ie);
-    GL_ALLOC(k_ie2, sizeof(uint64_t) * m_ie);
+    GL_CUDA(alloc16(k_ie, m_ie));
+    GL_CUDA(alloc16(k_ie2, m_ie));
     if (edata_bytes) {
-      GL_ALLOC(w_ie, (size_t) edata_bytes * m_ie + 64);
-      GL_ALLOC(w_ie2, (size_t) edata_bytes * m_ie + 64);
+      GL_CUDA(alloc16(w_ie, (size_t) edata_bytes * m_ie + 64));
+      GL_CUDA(alloc16(w_ie2, (size_t) edata_bytes * m_ie + 64));
     }
   }
   size_t ci = 0;
   for (uint64_t first = 0; first < E; first += CH, ++ci) {
     uint32_t cnt = (uint32_t) std::min<uint64_t>(CH, E - first);
-    GL_TRY(prod.fill(first, cnt, bs.as<uint32_t>(), bd.as<uint32_t>(), bw.p));
-    GL_CUDA(cudaMemsetAsync(c_oe.p, 0, sizeof(uint32_t) * (cnt + 1)));
-    GL_CUDA(cudaMemsetAsync(c_ie.p, 0, sizeof(uint32_t) * (cnt + 1)));
-    k_count<<<nblk(cnt), 256>>>(bs.as<uint32_t>(), bd.as<uint32_t>(), cnt, p,
-                                directed, c_oe.as<uint32_t>(), c_ie.as<uint32_t>());
+    GL_TRY(prod.fill(first, cnt, bs.get(), bd.get(), bw.get()));
+    GL_CUDA(cudaMemsetAsync(c_oe.get(), 0, sizeof(uint32_t) * (cnt + 1)));
+    GL_CUDA(cudaMemsetAsync(c_ie.get(), 0, sizeof(uint32_t) * (cnt + 1)));
+    k_count<<<nblk(cnt), 256>>>(bs.get(), bd.get(), cnt, p,
+                                directed, c_oe.get(), c_ie.get());
     GL_COUNT_LAUNCH();
-    GL_CUDA(cub::DeviceScan::ExclusiveSum(scan_tmp.p, scan_bytes, c_oe.as<uint32_t>(),
-                                          c_oe.as<uint32_t>(), (int) (cnt + 1)));
-    GL_CUDA(cub::DeviceScan::ExclusiveSum(scan_tmp.p, scan_bytes, c_ie.as<uint32_t>(),
-                                          c_ie.as<uint32_t>(), (int) (cnt + 1)));
+    GL_CUDA(cub::DeviceScan::ExclusiveSum(scan_tmp.get(), scan_bytes, c_oe.get(),
+                                          c_oe.get(), (int) (cnt + 1)));
+    GL_CUDA(cub::DeviceScan::ExclusiveSum(scan_tmp.get(), scan_bytes, c_ie.get(),
+                                          c_ie.get(), (int) (cnt + 1)));
     if (edata_bytes == 8) {
       k_emit<double><<<nblk(cnt), 256>>>(
-          bs.as<uint32_t>(), bd.as<uint32_t>(), bw.as<double>(), cnt, p, directed,
-          c_oe.as<uint32_t>(), c_ie.as<uint32_t>(), base_oe[ci], base_ie[ci],
-          k_oe.as<uint64_t>(), w_oe.as<double>(), k_ie.as<uint64_t>(), w_ie.as<double>());
+          bs.get(), bd.get(), (double*) bw.get(), cnt, p, directed,
+          c_oe.get(), c_ie.get(), base_oe[ci], base_ie[ci],
+          k_oe.get(), (double*) w_oe.get(), k_ie.get(), (double*) w_ie.get());
     } else {
       k_emit<float><<<nblk(cnt), 256>>>(
-          bs.as<uint32_t>(), bd.as<uint32_t>(), bw.as<float>(), cnt, p, directed,
-          c_oe.as<uint32_t>(), c_ie.as<uint32_t>(), base_oe[ci], base_ie[ci],
-          k_oe.as<uint64_t>(), w_oe.as<float>(), k_ie.as<uint64_t>(), w_ie.as<float>());
+          bs.get(), bd.get(), (float*) bw.get(), cnt, p, directed,
+          c_oe.get(), c_ie.get(), base_oe[ci], base_ie[ci],
+          k_oe.get(), (float*) w_oe.get(), k_ie.get(), (float*) w_ie.get());
     }
     GL_COUNT_LAUNCH();
     GL_CUDA(cudaGetLastError());
   }
   GL_CUDA(cudaDeviceSynchronize());
   // free chunk scratch before the big sorts
-  cudaFree(bs.release());
-  cudaFree(bd.release());
-  if (bw.p) cudaFree(bw.release());
-  cudaFree(c_oe.release());
-  cudaFree(c_ie.release());
+  bs.reset();
+  bd.reset();
+  bw.reset();
+  c_oe.reset();
+  c_ie.reset();
 
   const int end_bit = 32 + bits_for(f->ivnum);
   {
-    uint64_t *a = k_oe.as<uint64_t>(), *b = k_oe2.as<uint64_t>();
-    void *va = w_oe.p, *vb = w_oe2.p;
+    uint64_t *a = k_oe, *b = k_oe2;
+    void *va = w_oe, *vb = w_oe2;
     GL_TRY(sort_keys_u64(a, b, va, vb, edata_bytes, m_oe, end_bit));
-    k_oe.p = a; k_oe2.p = b; w_oe.p = va; w_oe2.p = vb;
+    if (a != k_oe.get()) std::swap(k_oe, k_oe2);
+    if (va != w_oe.get()) std::swap(w_oe, w_oe2);
   }
   if (directed) {
-    uint64_t *a = k_ie.as<uint64_t>(), *b = k_ie2.as<uint64_t>();
-    void *va = w_ie.p, *vb = w_ie2.p;
+    uint64_t *a = k_ie, *b = k_ie2;
+    void *va = w_ie, *vb = w_ie2;
     GL_TRY(sort_keys_u64(a, b, va, vb, edata_bytes, m_ie, end_bit));
-    k_ie.p = a; k_ie2.p = b; w_ie.p = va; w_ie2.p = vb;
+    if (a != k_ie.get()) std::swap(k_ie, k_ie2);
+    if (va != w_ie.get()) std::swap(w_ie, w_ie2);
   }
-  cudaFree(k_oe2.release());
-  if (w_oe2.p) cudaFree(w_oe2.release());
-  if (k_ie2.p) cudaFree(k_ie2.release());
-  if (w_ie2.p) cudaFree(w_ie2.release());
+  k_oe2.reset();
+  w_oe2.reset();
+  k_ie2.reset();
+  w_ie2.reset();
 
   // outer vertex set = distinct neighbours with the outer bit (both CSRs)
-  DevBuf outer_sorted;
+  DevBuf<uint32_t> outer_sorted;
   uint32_t ovnum = 0;
   if (f->fnum > 1) {
     uint64_t m_all = m_oe + m_ie;
-    DevBuf cand, flag, sel, nsel, tmp;
-    GL_ALLOC(cand, sizeof(uint32_t) * m_all);
-    GL_ALLOC(flag, m_all);
-    GL_ALLOC(sel, sizeof(uint32_t) * m_all);
-    GL_ALLOC(nsel, sizeof(uint64_t));
-    if (m_oe) k_outer_flags<<<nblk(m_oe), 256>>>(k_oe.as<uint64_t>(), m_oe, cand.as<uint32_t>(), flag.as<uint8_t>());
-    if (m_ie) k_outer_flags<<<nblk(m_ie), 256>>>(k_ie.as<uint64_t>(), m_ie, cand.as<uint32_t>() + m_oe, flag.as<uint8_t>() + m_oe);
+    DevBuf<uint32_t> cand, sel;
+    DevBuf<uint8_t> flag;
+    DevBuf<uint64_t> nsel;
+    DevBuf<char> tmp;
+    GL_CUDA(alloc16(cand, m_all));
+    GL_CUDA(alloc16(flag, m_all));
+    GL_CUDA(alloc16(sel, m_all));
+    GL_CUDA(alloc16(nsel, 1));
+    if (m_oe) k_outer_flags<<<nblk(m_oe), 256>>>(k_oe.get(), m_oe, cand.get(), flag.get());
+    if (m_ie) k_outer_flags<<<nblk(m_ie), 256>>>(k_ie.get(), m_ie, cand.get() + m_oe, flag.get() + m_oe);
     GL_COUNT_LAUNCH();
     size_t tb = 0;
-    GL_CUDA(cub::DeviceSelect::Flagged(nullptr, tb, cand.as<uint32_t>(), flag.as<uint8_t>(), sel.as<uint32_t>(), nsel.as<uint64_t>(), (int64_t) m_all));
-    GL_ALLOC(tmp, tb);
-    GL_CUDA(cub::DeviceSelect::Flagged(tmp.p, tb, cand.as<uint32_t>(), flag.as<uint8_t>(), sel.as<uint32_t>(), nsel.as<uint64_t>(), (int64_t) m_all));
+    GL_CUDA(cub::DeviceSelect::Flagged(nullptr, tb, cand.get(), flag.get(), sel.get(), nsel.get(), (int64_t) m_all));
+    GL_CUDA(alloc16(tmp, tb));
+    GL_CUDA(cub::DeviceSelect::Flagged(tmp.get(), tb, cand.get(), flag.get(), sel.get(), nsel.get(), (int64_t) m_all));
     uint64_t n_out = 0;
-    GL_CUDA(cudaMemcpy(&n_out, nsel.p, 8, cudaMemcpyDeviceToHost));
-    cudaFree(flag.release());
-    cudaFree(tmp.release());
+    GL_CUDA(cudaMemcpy(&n_out, nsel.get(), 8, cudaMemcpyDeviceToHost));
+    flag.reset();
+    tmp.reset();
     if (n_out) {
       // sort + unique
       size_t sb = 0;
-      cub::DoubleBuffer<uint32_t> db(sel.as<uint32_t>(), cand.as<uint32_t>());
+      cub::DoubleBuffer<uint32_t> db(sel.get(), cand.get());
       GL_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, sb, db, (int64_t) n_out, 0, bits_for(n)));
-      DevBuf st;
-      GL_ALLOC(st, sb);
-      GL_CUDA(cub::DeviceRadixSort::SortKeys(st.p, sb, db, (int64_t) n_out, 0, bits_for(n)));
+      DevBuf<char> st;
+      GL_CUDA(alloc16(st, sb));
+      GL_CUDA(cub::DeviceRadixSort::SortKeys(st.get(), sb, db, (int64_t) n_out, 0, bits_for(n)));
       uint32_t* sorted = db.Current();
       uint32_t* other = db.Alternate();
       size_t ub = 0;
-      GL_CUDA(cub::DeviceSelect::Unique(nullptr, ub, sorted, other, nsel.as<uint64_t>(), (int64_t) n_out));
-      DevBuf ut;
-      GL_ALLOC(ut, ub);
-      GL_CUDA(cub::DeviceSelect::Unique(ut.p, ub, sorted, other, nsel.as<uint64_t>(), (int64_t) n_out));
+      GL_CUDA(cub::DeviceSelect::Unique(nullptr, ub, sorted, other, nsel.get(), (int64_t) n_out));
+      DevBuf<char> ut;
+      GL_CUDA(alloc16(ut, ub));
+      GL_CUDA(cub::DeviceSelect::Unique(ut.get(), ub, sorted, other, nsel.get(), (int64_t) n_out));
       uint64_t nu = 0;
-      GL_CUDA(cudaMemcpy(&nu, nsel.p, 8, cudaMemcpyDeviceToHost));
+      GL_CUDA(cudaMemcpy(&nu, nsel.get(), 8, cudaMemcpyDeviceToHost));
       ovnum = (uint32_t) nu;
-      GL_ALLOC(outer_sorted, sizeof(uint32_t) * nu);
-      GL_CUDA(cudaMemcpy(outer_sorted.p, other, sizeof(uint32_t) * nu, cudaMemcpyDeviceToDevice));
+      GL_CUDA(alloc16(outer_sorted, nu));
+      GL_CUDA(cudaMemcpy(outer_sorted.get(), other, sizeof(uint32_t) * nu, cudaMemcpyDeviceToDevice));
     }
   }
   f->ovnum = ovnum;
   GL_ARG((uint64_t) f->ivnum + ovnum < (1ull << 32), "too many local vertices");
 
-  auto finish_csr = [&](DevBuf& keys, DevBuf& w, uint64_t m, DevCsr& out) -> int {
+  auto finish_csr = [&](DevBuf<uint64_t>& keys, DevBuf<char>& w, uint64_t m, DevCsr& out) -> int {
     out.rows = f->ivnum;
     out.entries = m;
     GL_CUDA(cudaMalloc(&out.rp, sizeof(uint64_t) * ((size_t) f->ivnum + 1)));
     GL_CUDA(cudaMalloc(&out.split, sizeof(uint64_t) * std::max<size_t>(f->ivnum, 1)));
     GL_CUDA(cudaMalloc(&out.col, sizeof(uint32_t) * (m + 16)));
-    k_rowptr<<<nblk((uint64_t) f->ivnum + 1), 256>>>(keys.as<uint64_t>(), m, f->ivnum, out.rp, out.split);
-    if (m) k_cols<<<nblk(m), 256>>>(keys.as<uint64_t>(), m, f->ivnum, outer_sorted.as<uint32_t>(), ovnum, out.col);
+    k_rowptr<<<nblk((uint64_t) f->ivnum + 1), 256>>>(keys.get(), m, f->ivnum, out.rp, out.split);
+    if (m) k_cols<<<nblk(m), 256>>>(keys.get(), m, f->ivnum, outer_sorted.get(), ovnum, out.col);
     GL_COUNT_LAUNCH();
     GL_CUDA(cudaDeviceSynchronize());
     out.w = w.release();
     f->device_bytes += sizeof(uint64_t) * (2 * (size_t) f->ivnum + 1) + sizeof(uint32_t) * m + (size_t) edata_bytes * m;
-    cudaFree(keys.release());
+    keys.reset();
     return GL_OK;
   };
   GL_TRY(finish_csr(k_oe, w_oe, m_oe, f->oe));
@@ -549,7 +545,7 @@ int build_from_producer(gl_frag* f, Producer& prod, uint64_t n, int directed,
   }
   if (ovnum) {
     GL_CUDA(cudaMalloc(&f->ovgid, sizeof(uint32_t) * ovnum));
-    k_ovgid<<<nblk(ovnum), 256>>>(outer_sorted.as<uint32_t>(), ovnum, p.chunk, f->fid_offset, f->ovgid);
+    k_ovgid<<<nblk(ovnum), 256>>>(outer_sorted.get(), ovnum, p.chunk, f->fid_offset, f->ovgid);
     GL_COUNT_LAUNCH();
     f->device_bytes += sizeof(uint32_t) * ovnum;
   }
@@ -567,15 +563,15 @@ int finish_common(gl_frag* f) {
   size_t words = ((size_t) f->ivnum + 31) / 32;
   GL_CUDA(cudaMalloc(&f->nonzero_deg, sizeof(uint32_t) * std::max<size_t>(words, 1)));
   GL_CUDA(cudaMemset(f->nonzero_deg, 0, sizeof(uint32_t) * std::max<size_t>(words, 1)));
-  DevBuf best;
-  GL_ALLOC(best, 8);
-  GL_CUDA(cudaMemset(best.p, 0, 8));
+  DevBuf<unsigned long long> best;
+  GL_CUDA(alloc16(best, 1));
+  GL_CUDA(cudaMemset(best.get(), 0, 8));
   if (f->ivnum) {
-    k_degree_stats<<<nblk(((uint64_t) f->ivnum + 31) / 32 * 32), 256>>>(f->oe.rp, f->ivnum, best.as<unsigned long long>(), f->nonzero_deg);
+    k_degree_stats<<<nblk(((uint64_t) f->ivnum + 31) / 32 * 32), 256>>>(f->oe.rp, f->ivnum, best.get(), f->nonzero_deg);
     GL_COUNT_LAUNCH();
   }
   unsigned long long hb = 0;
-  GL_CUDA(cudaMemcpy(&hb, best.p, 8, cudaMemcpyDeviceToHost));
+  GL_CUDA(cudaMemcpy(&hb, best.get(), 8, cudaMemcpyDeviceToHost));
   f->max_degree = (uint32_t) (hb >> 32);
   f->max_degree_lid = f->ivnum ? 0xFFFFFFFFu - (uint32_t) hb : 0;
   f->device_bytes += words * 4;
@@ -593,36 +589,36 @@ int finish_common(gl_frag* f) {
 int build_ovie(gl_frag* f) {
   // entries of oe whose neighbour is outer: count per row, scan, emit, sort
   const uint32_t rows = f->ivnum;
-  DevBuf cnt, pos, tmp;
-  GL_ALLOC(cnt, sizeof(uint64_t) * ((size_t) rows + 1));
-  GL_ALLOC(pos, sizeof(uint64_t) * ((size_t) rows + 1));
-  GL_CUDA(cudaMemset(cnt.p, 0, sizeof(uint64_t) * ((size_t) rows + 1)));
-  k_outer_deg<<<nblk(rows), 256>>>(f->oe.rp, f->oe.split, rows, cnt.as<uint64_t>());
+  DevBuf<uint64_t> cnt, pos;
+  DevBuf<char> tmp;
+  GL_CUDA(alloc16(cnt, ((size_t) rows + 1)));
+  GL_CUDA(alloc16(pos, ((size_t) rows + 1)));
+  GL_CUDA(cudaMemset(cnt.get(), 0, sizeof(uint64_t) * ((size_t) rows + 1)));
+  k_outer_deg<<<nblk(rows), 256>>>(f->oe.rp, f->oe.split, rows, cnt.get());
   GL_COUNT_LAUNCH();
   size_t tb = 0;
-  GL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt.as<uint64_t>(), pos.as<uint64_t>(), (int) (rows + 1)));
-  GL_ALLOC(tmp, tb);
-  GL_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, cnt.as<uint64_t>(), pos.as<uint64_t>(), (int) (rows + 1)));
+  GL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt.get(), pos.get(), (int) (rows + 1)));
+  GL_CUDA(alloc16(tmp, tb));
+  GL_CUDA(cub::DeviceScan::ExclusiveSum(tmp.get(), tb, cnt.get(), pos.get(), (int) (rows + 1)));
   uint64_t m = 0;
-  GL_CUDA(cudaMemcpy(&m, pos.as<uint64_t>() + rows, 8, cudaMemcpyDeviceToHost));
-  DevBuf keys, keys2;
-  GL_ALLOC(keys, sizeof(uint64_t) * m);
-  GL_ALLOC(keys2, sizeof(uint64_t) * m);
-  k_ovie_keys<<<nblk(rows), 256>>>(f->oe.rp, rows, f->oe.col, f->oe.split, f->ivnum, pos.as<uint64_t>(), keys.as<uint64_t>());
+  GL_CUDA(cudaMemcpy(&m, pos.get() + rows, 8, cudaMemcpyDeviceToHost));
+  DevBuf<uint64_t> keys, keys2;
+  GL_CUDA(alloc16(keys, m));
+  GL_CUDA(alloc16(keys2, m));
+  k_ovie_keys<<<nblk(rows), 256>>>(f->oe.rp, rows, f->oe.col, f->oe.split, f->ivnum, pos.get(), keys.get());
   GL_COUNT_LAUNCH();
-  uint64_t *a = keys.as<uint64_t>(), *b = keys2.as<uint64_t>();
+  uint64_t *a = keys, *b = keys2;
   void *va = nullptr, *vb = nullptr;
   GL_TRY(sort_keys_u64(a, b, va, vb, 0, m, 32 + bits_for(f->ovnum)));
-  keys.p = a;
-  keys2.p = b;
+  if (a != keys.get()) std::swap(keys, keys2);
   DevCsr& o = f->ovie;
   o.rows = f->ovnum;
   o.entries = m;
   GL_CUDA(cudaMalloc(&o.rp, sizeof(uint64_t) * ((size_t) f->ovnum + 1)));
   GL_CUDA(cudaMalloc(&o.split, sizeof(uint64_t) * std::max<size_t>(f->ovnum, 1)));
   GL_CUDA(cudaMalloc(&o.col, sizeof(uint32_t) * (m + 16)));
-  k_rowptr<<<nblk((uint64_t) f->ovnum + 1), 256>>>(keys.as<uint64_t>(), m, f->ovnum, o.rp, o.split);
-  if (m) k_low32<<<nblk(m), 256>>>(keys.as<uint64_t>(), m, o.col);
+  k_rowptr<<<nblk((uint64_t) f->ovnum + 1), 256>>>(keys.get(), m, f->ovnum, o.rp, o.split);
+  if (m) k_low32<<<nblk(m), 256>>>(keys.get(), m, o.col);
   GL_COUNT_LAUNCH();
   GL_CUDA(cudaDeviceSynchronize());
   f->device_bytes += sizeof(uint64_t) * ((size_t) f->ovnum + 1) + sizeof(uint32_t) * m;
@@ -717,15 +713,15 @@ int gl_frag_build_from_edges(gl_frag_t** out, const gl_edges_desc* d) {
   f->load_strategy = d->load_strategy;
   HostProducer prod;
   prod.d = d;
-  DevBuf d_oids;
+  DevBuf<int64_t> d_oids;
   if (d->oids) {
-    if (cudaMalloc(&d_oids.p, sizeof(int64_t) * std::max<uint64_t>(d->n_vertices, 1)) != cudaSuccess ||
-        cudaMemcpy(d_oids.p, d->oids, sizeof(int64_t) * d->n_vertices, cudaMemcpyHostToDevice) != cudaSuccess) {
+    if (d_oids.alloc(std::max<uint64_t>(d->n_vertices, 1)) != cudaSuccess ||
+        cudaMemcpy(d_oids, d->oids, sizeof(int64_t) * d->n_vertices, cudaMemcpyHostToDevice) != cudaSuccess) {
       set_error("oid upload failed");
       delete f;
       return GL_ERR_CUDA;
     }
-    prod.d_oids = d_oids.as<int64_t>();
+    prod.d_oids = d_oids;
   }
   int st = build_from_producer(f, prod, d->n_vertices, d->directed ? 1 : 0,
                                d->edata ? d->edata_bytes : 0);

@@ -50,100 +50,96 @@ k_perm_rows(const uint64_t* __restrict__ rp, const uint32_t* __restrict__ col,
 }
 }  // namespace
 
-int build_hub_order(cudaStream_t s, const uint64_t* rp, uint32_t n, uint32_t** perm_out, uint32_t** order_out) {
-  uint32_t *key = nullptr, *key2 = nullptr, *val = nullptr, *val2 = nullptr;
-  GL_CUDA(cudaMalloc(&key, 4ull * std::max<uint32_t>(n, 1)));
-  GL_CUDA(cudaMalloc(&key2, 4ull * std::max<uint32_t>(n, 1)));
-  GL_CUDA(cudaMalloc(&val, 4ull * std::max<uint32_t>(n, 1)));
-  GL_CUDA(cudaMalloc(&val2, 4ull * std::max<uint32_t>(n, 1)));
+int build_hub_order(cudaStream_t s, const uint64_t* rp, uint32_t n, DevBuf<uint32_t>* perm_out, DevBuf<uint32_t>* order_out) {
+  DevBuf<uint32_t> key, key2, val, val2, perm;
+  DevBuf<char> tmp;
+  GL_CUDA(key.alloc(std::max<uint32_t>(n, 1)));
+  GL_CUDA(key2.alloc(std::max<uint32_t>(n, 1)));
+  GL_CUDA(val.alloc(std::max<uint32_t>(n, 1)));
+  GL_CUDA(val2.alloc(std::max<uint32_t>(n, 1)));
   if (n) GL_LAUNCH(k_degkey, (n + 255) / 256, 256, s, rp, n, key, val);
   size_t tb = 0;
   cub::DoubleBuffer<uint32_t> kb(key, key2), vb(val, val2);
   GL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, kb, vb, (int) n, 0, 32, s));
-  void* tmp = nullptr;
-  GL_CUDA(cudaMalloc(&tmp, std::max<size_t>(tb, 16)));
+  GL_CUDA(tmp.alloc(std::max<size_t>(tb, 16)));
   if (n) GL_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, kb, vb, (int) n, 0, 32, s));
-  uint32_t* perm = nullptr;
-  GL_CUDA(cudaMalloc(&perm, 4ull * std::max<uint32_t>(n, 1)));
+  GL_CUDA(perm.alloc(std::max<uint32_t>(n, 1)));
   if (n) GL_LAUNCH(k_invert, (n + 255) / 256, 256, s, vb.Current(), n, perm);
   GL_CUDA(cudaStreamSynchronize(s));
-  uint32_t* order = vb.Current();
-  cudaFree(key);
-  cudaFree(key2);
-  cudaFree(vb.Alternate());
-  cudaFree(tmp);
-  *perm_out = perm;
-  if (order_out) *order_out = order; else cudaFree(order);
+  DevBuf<uint32_t>& order = vb.Current() == val.get() ? val : val2;
+  // the temporaries are freed in allocation order
+  key.reset();
+  key2.reset();
+  (&order == &val ? val2 : val).reset();
+  tmp.reset();
+  *perm_out = std::move(perm);
+  if (order_out) *order_out = std::move(order);
   return GL_OK;
 }
 
 // rows reordered by `order`, neighbours relabelled by `perm`
 int build_permuted_csr(cudaStream_t s, const uint64_t* rp, const uint32_t* col, uint64_t m, uint32_t n,
-                       const uint32_t* order, const uint32_t* perm, uint64_t** rp_out, uint32_t** col_out,
-                       const void* w4, void** w4_out, bool sort_rows) {
-  uint64_t *deg = nullptr, *rp_p = nullptr;
-  GL_CUDA(cudaMalloc(&deg, 8ull * ((size_t) n + 1)));
-  GL_CUDA(cudaMalloc(&rp_p, 8ull * ((size_t) n + 1)));
+                       const uint32_t* order, const uint32_t* perm, DevBuf<uint64_t>* rp_out, DevBuf<uint32_t>* col_out,
+                       const void* w4, DevBuf<uint32_t>* w4_out, bool sort_rows) {
+  DevBuf<uint64_t> deg, rp_p;
+  GL_CUDA(deg.alloc((size_t) n + 1));
+  GL_CUDA(rp_p.alloc((size_t) n + 1));
   GL_LAUNCH(k_perm_deg, (n + 1 + 255) / 256, 256, s, rp, order, n, deg);
   size_t tb = 0;
-  GL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, deg, rp_p, (int) (n + 1), s));
-  void* tmp = nullptr;
-  GL_CUDA(cudaMalloc(&tmp, std::max<size_t>(tb, 16)));
-  GL_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, deg, rp_p, (int) (n + 1), s));
-  uint32_t* col_p = nullptr;
-  GL_CUDA(cudaMalloc(&col_p, 4ull * (m + 16)));
-  uint32_t* w_p = nullptr;
-  if (w4) GL_CUDA(cudaMalloc(&w_p, 4ull * (m + 16)));
+  GL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, deg.get(), rp_p.get(), (int) (n + 1), s));
+  DevBuf<char> tmp;
+  GL_CUDA(tmp.alloc(std::max<size_t>(tb, 16)));
+  GL_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, deg.get(), rp_p.get(), (int) (n + 1), s));
+  DevBuf<uint32_t> col_p, w_p;
+  GL_CUDA(col_p.alloc(m + 16));
+  if (w4) GL_CUDA(w_p.alloc(m + 16));
   if (n) GL_LAUNCH(k_perm_rows, num_sms() * 8, 256, s, rp, col, order, perm, n, rp_p, col_p, (const uint32_t*) w4, w_p);
   // rows sorted by the new ids = by descending degree of the neighbour: the
   // most promising parents come first in a pull scan, and the entries of a
   // row that fall into the same bitmap word are adjacent
   if (n && m && sort_rows) {
-    uint32_t* sorted = nullptr;
-    GL_CUDA(cudaMalloc(&sorted, 4ull * (m + 16)));
+    DevBuf<uint32_t> sorted;
+    GL_CUDA(sorted.alloc(m + 16));
     size_t sb = 0;
-    void* st = nullptr;
+    DevBuf<char> st;
     if (!w_p) {
-      GL_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, sb, col_p, sorted, (int64_t) m, (int64_t) n, rp_p, rp_p + 1, s));
-      GL_CUDA(cudaMalloc(&st, std::max<size_t>(sb, 16)));
-      GL_CUDA(cub::DeviceSegmentedSort::SortKeys(st, sb, col_p, sorted, (int64_t) m, (int64_t) n, rp_p, rp_p + 1, s));
+      GL_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, sb, col_p.get(), sorted.get(), (int64_t) m, (int64_t) n, rp_p.get(), rp_p + 1, s));
+      GL_CUDA(st.alloc(std::max<size_t>(sb, 16)));
+      GL_CUDA(cub::DeviceSegmentedSort::SortKeys(st, sb, col_p.get(), sorted.get(), (int64_t) m, (int64_t) n, rp_p.get(), rp_p + 1, s));
     } else {
-      uint32_t* w_sorted = nullptr;
-      GL_CUDA(cudaMalloc(&w_sorted, 4ull * (m + 16)));
-      GL_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, sb, col_p, sorted, w_p, w_sorted, (int64_t) m, (int64_t) n, rp_p, rp_p + 1, s));
-      GL_CUDA(cudaMalloc(&st, std::max<size_t>(sb, 16)));
-      GL_CUDA(cub::DeviceSegmentedSort::SortPairs(st, sb, col_p, sorted, w_p, w_sorted, (int64_t) m, (int64_t) n, rp_p, rp_p + 1, s));
+      DevBuf<uint32_t> w_sorted;
+      GL_CUDA(w_sorted.alloc(m + 16));
+      GL_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, sb, col_p.get(), sorted.get(), w_p.get(), w_sorted.get(), (int64_t) m, (int64_t) n, rp_p.get(), rp_p + 1, s));
+      GL_CUDA(st.alloc(std::max<size_t>(sb, 16)));
+      GL_CUDA(cub::DeviceSegmentedSort::SortPairs(st, sb, col_p.get(), sorted.get(), w_p.get(), w_sorted.get(), (int64_t) m, (int64_t) n, rp_p.get(), rp_p + 1, s));
       GL_CUDA(cudaStreamSynchronize(s));
-      cudaFree(w_p);
-      w_p = w_sorted;
+      w_p = std::move(w_sorted);
     }
     GL_CUDA(cudaStreamSynchronize(s));
-    cudaFree(st);
-    cudaFree(col_p);
-    col_p = sorted;
+    st.reset();
+    col_p = std::move(sorted);
   }
   GL_CUDA(cudaStreamSynchronize(s));
-  cudaFree(deg);
-  cudaFree(tmp);
-  *rp_out = rp_p;
-  *col_out = col_p;
-  if (w4_out) *w4_out = w_p;
+  deg.reset();
+  tmp.reset();
+  *rp_out = std::move(rp_p);
+  *col_out = std::move(col_p);
+  if (w4_out) *w4_out = std::move(w_p);
   return GL_OK;
 }
 
-int sort_csr_rows(cudaStream_t s, const uint64_t* rp, uint32_t n, uint64_t m, uint32_t** col) {
+int sort_csr_rows(cudaStream_t s, const uint64_t* rp, uint32_t n, uint64_t m, DevBuf<uint32_t>* col) {
   if (!n || !m) return GL_OK;
-  uint32_t* sorted = nullptr;
-  GL_CUDA(cudaMalloc(&sorted, 4ull * (m + 16)));
+  DevBuf<uint32_t> sorted;
+  GL_CUDA(sorted.alloc(m + 16));
   size_t sb = 0;
-  void* st = nullptr;
-  GL_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, sb, *col, sorted, (int64_t) m, (int64_t) n, rp, rp + 1, s));
-  GL_CUDA(cudaMalloc(&st, std::max<size_t>(sb, 16)));
-  GL_CUDA(cub::DeviceSegmentedSort::SortKeys(st, sb, *col, sorted, (int64_t) m, (int64_t) n, rp, rp + 1, s));
+  DevBuf<char> st;
+  GL_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, sb, col->get(), sorted.get(), (int64_t) m, (int64_t) n, rp, rp + 1, s));
+  GL_CUDA(st.alloc(std::max<size_t>(sb, 16)));
+  GL_CUDA(cub::DeviceSegmentedSort::SortKeys(st, sb, col->get(), sorted.get(), (int64_t) m, (int64_t) n, rp, rp + 1, s));
   GL_CUDA(cudaStreamSynchronize(s));
-  cudaFree(st);
-  cudaFree(*col);
-  *col = sorted;
+  st.reset();
+  *col = std::move(sorted);
   return GL_OK;
 }
 

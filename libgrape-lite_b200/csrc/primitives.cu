@@ -238,15 +238,14 @@ int gl_compact_bitmap(void* stream, const uint32_t* bitmap, uint32_t n_bits,
   cudaStream_t s = (cudaStream_t) stream;
   DeviceInfo* di;
   GL_TRY(device_info(&di));
-  uint32_t* d_count = nullptr;
-  GL_CUDA(cudaMalloc(&d_count, 4));
+  DevBuf<uint32_t> d_count;
+  GL_CUDA(d_count.alloc(1));
   GL_CUDA(cudaMemsetAsync(d_count, 0, 4, s));
   int g = std::max(1, std::min<int>(di->sm_count * 8, (int) ((n_bits + kTB - 1) / kTB)));
   k_compact<<<g, kTB, 0, s>>>(bitmap, n_bits, queue_out, d_count);
   GL_COUNT_LAUNCH();
   cudaError_t e = cudaMemcpyAsync(count_host, d_count, 4, cudaMemcpyDeviceToHost, s);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  cudaFree(d_count);
   if (e != cudaSuccess) {
     set_error("gl_compact_bitmap: %s", cudaGetErrorString(e));
     return GL_ERR_CUDA;

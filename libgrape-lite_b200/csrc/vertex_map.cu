@@ -20,6 +20,7 @@
 
 #include <algorithm>
 #include <cstdio>
+#include <memory>
 #include <vector>
 
 #include "apps_common.cuh"
@@ -29,10 +30,10 @@ struct gl_vm {
   int fid_offset = 31;
   uint32_t id_mask = 0x7fffffffu;
   std::vector<uint64_t> off;   // [fnum+1]
-  int64_t* d_l2o = nullptr;    // [off[fnum]]
-  uint64_t* d_off = nullptr;   // [fnum+1]
-  int64_t* d_sorted_oid = nullptr;   // null when every slice of l2o is ascending
-  uint32_t* d_sorted_lid = nullptr;
+  gl::DevBuf<int64_t> d_l2o;    // [off[fnum]]
+  gl::DevBuf<uint64_t> d_off;   // [fnum+1]
+  gl::DevBuf<int64_t> d_sorted_oid;   // null when every slice of l2o is ascending
+  gl::DevBuf<uint32_t> d_sorted_lid;
 };
 
 namespace gl {
@@ -95,77 +96,70 @@ int gl_vm_create(gl_vm_t** out, uint32_t fnum, const uint64_t* ivnums, const int
   GL_ARG(out && ivnums && oids && fnum >= 1 && fnum <= GL_MAX_FNUM, "bad argument");
   DeviceInfo* di;
   GL_TRY(device_info(&di));
-  gl_vm* vm = new gl_vm;
+  std::unique_ptr<gl_vm> vm(new gl_vm);
   vm->fnum = fnum;
   id_parser_init(fnum, &vm->fid_offset, &vm->id_mask);
   vm->off.assign(fnum + 1, 0);
   for (uint32_t f = 0; f < fnum; ++f) vm->off[f + 1] = vm->off[f] + ivnums[f];
   const uint64_t total = vm->off[fnum];
-  auto fail = [&](int st) {
-    gl_vm_destroy(vm);
-    return st;
-  };
-  if (cudaMalloc(&vm->d_l2o, sizeof(int64_t) * std::max<uint64_t>(total, 1)) != cudaSuccess ||
-      cudaMalloc(&vm->d_off, sizeof(uint64_t) * (fnum + 1)) != cudaSuccess) {
+  if (vm->d_l2o.alloc(std::max<uint64_t>(total, 1)) != cudaSuccess || vm->d_off.alloc(fnum + 1) != cudaSuccess) {
     set_error("gl_vm_create: device allocation failed");
-    return fail(GL_ERR_NOMEM);
+    return GL_ERR_NOMEM;
   }
-  cudaMemcpy(vm->d_off, vm->off.data(), sizeof(uint64_t) * (fnum + 1), cudaMemcpyHostToDevice);
+  GL_CUDA(cudaMemcpy(vm->d_off, vm->off.data(), sizeof(uint64_t) * (fnum + 1), cudaMemcpyHostToDevice));
   for (uint32_t f = 0; f < fnum; ++f) {
     if (!ivnums[f]) continue;
     if (!oids[f]) {
       set_error("gl_vm_create: oid list of fragment %u is null", f);
-      return fail(GL_ERR_ARG);
+      return GL_ERR_ARG;
     }
     if (cudaMemcpy(vm->d_l2o + vm->off[f], oids[f], sizeof(int64_t) * ivnums[f], cudaMemcpyHostToDevice) != cudaSuccess) {
       set_error("gl_vm_create: upload failed");
-      return fail(GL_ERR_CUDA);
+      return GL_ERR_CUDA;
     }
   }
   // ascending slices need no side index
-  uint32_t* d_bad = nullptr;
   uint32_t bad = 0;
-  if (cudaMalloc(&d_bad, 4) != cudaSuccess) return fail(GL_ERR_NOMEM);
-  cudaMemset(d_bad, 0, 4);
-  if (total > 1) {
-    k_vm_check_sorted<<<num_sms() * 4, 256>>>(vm->d_l2o, vm->d_off, fnum, d_bad);
-    GL_COUNT_LAUNCH();
+  {
+    DevBuf<uint32_t> d_bad;
+    if (d_bad.alloc(1) != cudaSuccess) return GL_ERR_NOMEM;
+    GL_CUDA(cudaMemset(d_bad, 0, 4));
+    if (total > 1) {
+      k_vm_check_sorted<<<num_sms() * 4, 256>>>(vm->d_l2o, vm->d_off, fnum, d_bad);
+      GL_COUNT_LAUNCH();
+    }
+    GL_CUDA(cudaMemcpy(&bad, d_bad, 4, cudaMemcpyDeviceToHost));
   }
-  cudaMemcpy(&bad, d_bad, 4, cudaMemcpyDeviceToHost);
-  cudaFree(d_bad);
   if (bad) {
     // per-slice sort of (oid, lid): one segmented radix sort
-    int64_t* k_in = vm->d_l2o;
-    uint32_t* v_in = nullptr;
-    if (cudaMalloc(&vm->d_sorted_oid, sizeof(int64_t) * total) != cudaSuccess ||
-        cudaMalloc(&vm->d_sorted_lid, sizeof(uint32_t) * total) != cudaSuccess ||
-        cudaMalloc(&v_in, sizeof(uint32_t) * total) != cudaSuccess) {
-      cudaFree(v_in);
+    const int64_t* k_in = vm->d_l2o;
+    DevBuf<uint32_t> v_in;
+    if (vm->d_sorted_oid.alloc(total) != cudaSuccess || vm->d_sorted_lid.alloc(total) != cudaSuccess ||
+        v_in.alloc(total) != cudaSuccess) {
       set_error("gl_vm_create: device allocation failed");
-      return fail(GL_ERR_NOMEM);
+      return GL_ERR_NOMEM;
     }
     k_vm_iota<<<num_sms() * 4, 256>>>(v_in, vm->d_off, fnum);
     GL_COUNT_LAUNCH();
     size_t tb = 0;
-    cub::DeviceSegmentedRadixSort::SortPairs(nullptr, tb, k_in, vm->d_sorted_oid, v_in, vm->d_sorted_lid, (int) total,
-                                             (int) fnum, vm->d_off, vm->d_off + 1);
-    void* tmp = nullptr;
-    cudaMalloc(&tmp, std::max<size_t>(tb, 16));
-    cudaError_t e = cub::DeviceSegmentedRadixSort::SortPairs(tmp, tb, k_in, vm->d_sorted_oid, v_in, vm->d_sorted_lid,
-                                                             (int) total, (int) fnum, vm->d_off, vm->d_off + 1);
+    cub::DeviceSegmentedRadixSort::SortPairs(nullptr, tb, k_in, vm->d_sorted_oid.get(), v_in.get(), vm->d_sorted_lid.get(),
+                                             (int) total, (int) fnum, vm->d_off.get(), vm->d_off + 1);
+    DevBuf<char> tmp;
+    GL_CUDA(tmp.alloc(std::max<size_t>(tb, 16)));
+    cudaError_t e = cub::DeviceSegmentedRadixSort::SortPairs(tmp, tb, k_in, vm->d_sorted_oid.get(), v_in.get(),
+                                                             vm->d_sorted_lid.get(), (int) total, (int) fnum,
+                                                             vm->d_off.get(), vm->d_off + 1);
     cudaDeviceSynchronize();
-    cudaFree(tmp);
-    cudaFree(v_in);
     if (e != cudaSuccess) {
       set_error("gl_vm_create: segmented sort failed: %s", cudaGetErrorString(e));
-      return fail(GL_ERR_CUDA);
+      return GL_ERR_CUDA;
     }
   }
   if (cudaDeviceSynchronize() != cudaSuccess) {
     set_error("gl_vm_create: %s", cudaGetErrorString(cudaGetLastError()));
-    return fail(GL_ERR_CUDA);
+    return GL_ERR_CUDA;
   }
-  *out = vm;
+  *out = vm.release();
   return GL_OK;
 }
 
@@ -199,14 +193,7 @@ int gl_vm_gid2oid(const gl_vm_t* vm, void* stream, const uint32_t* d_gids, uint6
   return GL_OK;
 }
 
-void gl_vm_destroy(gl_vm_t* vm) {
-  if (!vm) return;
-  cudaFree(vm->d_l2o);
-  cudaFree(vm->d_off);
-  cudaFree(vm->d_sorted_oid);
-  cudaFree(vm->d_sorted_lid);
-  delete vm;
-}
+void gl_vm_destroy(gl_vm_t* vm) { delete vm; }
 
 // ---------------------------------------------------------------------------
 // on-disk fragment

@@ -10,26 +10,20 @@ int Engine::init(const gl_frag* f) {
   sm_count = di->sm_count;
   grid = sm_count * 8;
   GL_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-  GL_CUDA(cudaMalloc(&ctrl, sizeof(ScanCtrl)));
+  GL_CUDA(ctrl.alloc(1));
   GL_CUDA(cudaMemset(ctrl, 0, sizeof(ScanCtrl)));
-  GL_CUDA(cudaMallocHost(&h_ctrl, sizeof(ScanCtrl)));
+  GL_CUDA(h_ctrl.alloc(1));
   memset(h_ctrl, 0, sizeof(ScanCtrl));
   // every hub row has > hub_deg entries, so (#pieces) <= M/kHubChunk + M/hub_deg
   uint64_t m = std::max<uint64_t>(f->oe.entries, f->ie.entries);
   uint64_t cap = m / kHubChunk + m / std::max<uint32_t>(hub_deg, 1) + 1024;
   hub_cap = (uint32_t) std::min<uint64_t>(cap, 0x7FFFFFFFull);
-  GL_CUDA(cudaMalloc(&hubs, sizeof(HubItem) * (size_t) hub_cap));
+  GL_CUDA(hubs.alloc(hub_cap));
   return GL_OK;
 }
 
 void Engine::destroy() {
-  if (ctrl) cudaFree(ctrl);
-  if (h_ctrl) cudaFreeHost(h_ctrl);
-  if (hubs) cudaFree(hubs);
   if (stream) cudaStreamDestroy(stream);
-  ctrl = nullptr;
-  h_ctrl = nullptr;
-  hubs = nullptr;
   stream = nullptr;
 }
 
@@ -241,7 +235,6 @@ int gl_app_result_oids(gl_app_t* a, int64_t* host_out, size_t count) {
 void gl_app_destroy(gl_app_t* a) {
   if (!a) return;
   if (a->eng.stream) l2_persist_clear(a->eng.stream);   // give the L2 set-aside back (common.cu)
-  a->mm.Destroy();
   a->rec.destroy();
   a->eng.destroy();
   delete a;

@@ -82,8 +82,11 @@ def main():
         mm.close()
         return out, rounds, total
 
-    if os.environ.get("GL_SHAPES", "0") == "1":
-        run_shapes(pkg, gdist, pyoracle, rank, world, gather, failures)
+    if os.environ.get("GL_SHAPES", "0") == "1" or os.environ.get("GL_RESOURCES", "0") == "1":
+        if os.environ.get("GL_SHAPES", "0") == "1":
+            run_shapes(pkg, gdist, pyoracle, rank, world, gather, failures)
+        else:
+            run_resources(pkg, gdist, rank, world, scale, dist.barrier, failures)
         flag = torch.tensor([len(failures)], device=dev)
         dist.broadcast(flag, 0)
         dist.destroy_process_group()
@@ -208,6 +211,42 @@ def main():
     dist.broadcast(flag, 0)
     dist.destroy_process_group()
     sys.exit(1 if int(flag.item()) else 0)
+
+
+def run_resources(pkg, gdist, rank, world, scale, barrier, failures):
+    """GL_RESOURCES=1: every app configuration runs create -> query -> result -> destroy on its
+    fragment group once as warm-up and three more times; the free device memory (all ranks share
+    cuda:0) must end where the warm-up left it."""
+    frag = pkg.Fragment.rmat(scale, 16, seed=17, weight_mode=1, fid=rank, fnum=world)
+    comm = gdist.make_comm(rank, world, frag.ivnum)
+
+    def free_bytes():
+        torch.cuda.synchronize()
+        barrier()
+        f = torch.cuda.mem_get_info()[0]
+        barrier()
+        return f
+
+    configs = [("bfs", dict(source_oid=0, fuse_supersteps=1)), ("bfs", dict(source_oid=0, fuse_supersteps=0)),
+               ("sssp", dict(source_oid=0, sssp_f64=0)), ("sssp", dict(source_oid=0, sssp_f64=1)),
+               ("wcc", {}), ("wcc_opt", {}), ("pagerank", dict(pr_pull=0)), ("pagerank", dict(pr_pull=1)),
+               ("cdlp", dict(max_round=5)), ("lcc", {})]
+    for kind, cfg in configs:
+        frees = []
+        for it in range(4):
+            app = pkg.App(kind, frag, comm, **cfg)
+            app.query()
+            app.result()
+            app.close()
+            frees.append(free_bytes())
+        ok = frees[-1] == frees[0]
+        if rank == 0:
+            print("[mgpu] %-9s %-32s fnum=%d scale=%d free after cycles %s %s"
+                  % (kind, cfg, world, scale, frees, "RELEASED" if ok else "LEAKED"), flush=True)
+        if not ok:
+            failures.append(kind)
+    comm.close()
+    frag.close()
 
 
 def run_shapes(pkg, gdist, pyoracle, rank, world, gather, failures):
