@@ -391,14 +391,21 @@ typedef enum {
   GL_APP_PAGERANK = 3, /* cuda/pagerank/pagerank.h result: double              */
   GL_APP_CDLP = 4,     /* cuda/cdlp/cdlp.h      result: int64 label            */
   GL_APP_LCC = 5,      /* cuda/lcc/lcc_opt.h    result: double                 */
-  GL_APP_WCC_OPT = 6   /* cuda/wcc/wcc_opt.h (union-find) result: as GL_APP_WCC  */
+  GL_APP_WCC_OPT = 6,  /* cuda/wcc/wcc_opt.h (union-find) result: as GL_APP_WCC  */
+  /* undirected fragments only (GL_ERR_ARG otherwise); degree = CSR entries
+   * (a multi-edge counts once per copy, a self loop twice) */
+  GL_APP_CORE_DECOMPOSITION = 7, /* core_decomposition/core_decomposition.h
+                                    result: int64 core number (isolated: 0)     */
+  GL_APP_KCORE = 8     /* kcore/kcore.h  result: int64 entries whose other
+                          endpoint survives the k-core peel (k = max_round);
+                          v is in the k-core iff value >= k                   */
 } gl_app_kind;
 
 typedef struct {
   int lb;                /* gl_lb (AppConfig::lb, cuda/app_config.h:22-27)     */
   int64_t source_oid;    /* --bfs_source / --sssp_source                        */
   double pr_delta;       /* --pr_d                                              */
-  int max_round;         /* --pr_mr / --cdlp_mr                                 */
+  int max_round;         /* --pr_mr / --cdlp_mr; GL_APP_KCORE: k (--kcore_k)   */
   int sssp_f64;          /* 1: fp64 distances on device (real-weight 1e-6 run)  */
   double sssp_prio;      /* 0 -> reference heuristic 32*avg_w/avg_deg           */
   int direction_opt;     /* BFS: 0 push only, 1 push/pull (bfs.h:168-261)       */

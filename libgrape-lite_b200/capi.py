@@ -9,8 +9,10 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgrape_b200.so")
 
 GL_LB = {"none": 0, "cm": 1, "wm": 2, "cta": 3, "strict": 4, "cmold": 5}
-APP = {"bfs": 0, "sssp": 1, "wcc": 2, "pagerank": 3, "cdlp": 4, "lcc": 5, "wcc_opt": 6}
-RESULT_DTYPE = {0: np.int64, 1: np.float64, 2: np.int64, 3: np.float64, 4: np.int64, 5: np.float64, 6: np.int64}
+APP = {"bfs": 0, "sssp": 1, "wcc": 2, "pagerank": 3, "cdlp": 4, "lcc": 5, "wcc_opt": 6,
+       "core_decomposition": 7, "kcore": 8}
+RESULT_DTYPE = {0: np.int64, 1: np.float64, 2: np.int64, 3: np.float64, 4: np.int64, 5: np.float64, 6: np.int64,
+                7: np.int64, 8: np.int64}
 GL_MAX_STEP_STATS = 512
 GL_IPC_HANDLE_BYTES = 64
 
@@ -436,11 +438,16 @@ def bitmap_count(bitmap_dev, nbits):
 
 
 class App:
-    """One PIE app bound to a fragment (GPUWorker analogue)."""
+    """One PIE app bound to a fragment (GPUWorker analogue).  "kcore" takes its
+    k as App("kcore", frag, k=...) (carried in max_round); it has no default."""
 
     def __init__(self, kind, frag, comm=None, **cfg):
         self.kind = APP[kind] if isinstance(kind, str) else kind
         self.frag = frag
+        if self.kind == APP["kcore"]:
+            if "k" not in cfg:
+                raise GrapeError("kcore needs k: App('kcore', frag, k=...)")
+            cfg["max_round"] = int(cfg.pop("k"))
         c = AppConfig()
         lib().gl_app_config_default(C.byref(c))
         for k, v in cfg.items():

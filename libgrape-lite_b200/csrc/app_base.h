@@ -97,4 +97,6 @@ gl_app* make_pagerank();
 gl_app* make_cdlp();
 gl_app* make_lcc();
 gl_app* make_wcc_opt();
+gl_app* make_core_decomposition();
+gl_app* make_kcore();
 }  // namespace gl

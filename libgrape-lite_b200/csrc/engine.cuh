@@ -610,17 +610,15 @@ k_queue_scan_warp(Src q, uint32_t n, EdgeRange er,
   if (lane_id() == 0 && s) atomicAdd(&ctrl->scanned, s);
 }
 
-// LB cm / cta: a CTA takes kTileV queue entries per ticket and walks them with
-// the same tile walk as the frontier scan (cm keeps every row in the tile:
-// hub_deg = UINT32_MAX; cta defers long rows to k_hub_scan).
+// Queue scan phase: a CTA takes kTileV queue entries per ticket and walks them
+// with the same tile walk as the frontier scan; rows longer than hub_deg go to
+// the hub list.  A __device__ phase so that the stand-alone kernel
+// (k_queue_scan_cta) and fused whole-query kernels share it.
 template <class Op, class Src = ArraySrc>
-__global__ void __launch_bounds__(kTB)
-k_queue_scan_cta(Src q, uint32_t n, EdgeRange er,
-                 Op op, ScanCtrl* ctrl, HubItem* hubs, uint32_t hub_cap,
-                 uint32_t hub_deg) {
-  __shared__ ScanSmem<typename Op::Meta> sm;
+GL_DEV void queue_scan_phase(ScanSmem<typename Op::Meta>& sm, Src q, uint32_t n, EdgeRange er,
+                             const Op& op, ScanCtrl* ctrl, HubItem* hubs, uint32_t hub_cap,
+                             uint32_t hub_deg, ScanAcc& acc) {
   const uint32_t ntiles = (n + kTileV - 1) / kTileV;
-  ScanAcc acc;
   uint64_t scanned = 0;
   if (threadIdx.x == 0) sm.hubn = 0;
   __syncthreads();
@@ -635,9 +633,21 @@ k_queue_scan_cta(Src q, uint32_t n, EdgeRange er,
     __syncthreads();
     walk_tile<Op>(sm, nf, er, op, ctrl, hubs, hub_cap, hub_deg, acc, scanned);
   }
-  flush_acc(acc, ctrl);
   if (threadIdx.x == 0 && scanned)
     atomicAdd(&ctrl->scanned, (unsigned long long) scanned);
+}
+
+// LB cm / cta: the queue scan phase as a kernel (cm keeps every row in the
+// tile: hub_deg = UINT32_MAX; cta defers long rows to k_hub_scan).
+template <class Op, class Src = ArraySrc>
+__global__ void __launch_bounds__(kTB)
+k_queue_scan_cta(Src q, uint32_t n, EdgeRange er,
+                 Op op, ScanCtrl* ctrl, HubItem* hubs, uint32_t hub_cap,
+                 uint32_t hub_deg) {
+  __shared__ ScanSmem<typename Op::Meta> sm;
+  ScanAcc acc;
+  queue_scan_phase<Op, Src>(sm, q, n, er, op, ctrl, hubs, hub_cap, hub_deg, acc);
+  flush_acc(acc, ctrl);
 }
 
 // LB strict: exact edge balance.  pfx[i] = exclusive prefix of the queue's

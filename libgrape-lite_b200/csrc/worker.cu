@@ -118,6 +118,8 @@ int gl_app_create(gl_app_t** out, int kind, gl_frag_t* frag, gl_comm_t* comm,
     case GL_APP_CDLP: a = make_cdlp(); break;
     case GL_APP_LCC: a = make_lcc(); break;
     case GL_APP_WCC_OPT: a = make_wcc_opt(); break;
+    case GL_APP_CORE_DECOMPOSITION: a = make_core_decomposition(); break;
+    case GL_APP_KCORE: a = make_kcore(); break;
     default:
       set_error("unknown app kind %d", kind);
       return GL_ERR_ARG;
