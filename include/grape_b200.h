@@ -304,7 +304,8 @@ int gl_comm_peer_write_us(gl_comm_t*, size_t bytes, int vec16, int all_peers, in
  * counts, runs the device-side barrier + termination vote and flips the
  * double buffer; what was sent in round r is readable through recv_slot /
  * recv_bytes during round r+1 only (the reference's rule: messages are
- * visible in the next IncEval).  Termination = no fragment sent a byte and
+ * visible in the next IncEval); round 0 after gl_mm_start receives nothing.
+ * Termination = no fragment sent a byte and
  * none called force_continue (gpu_message_manager.h:413-430).
  * ------------------------------------------------------------------ */
 typedef struct gl_mm gl_mm_t;
@@ -376,7 +377,10 @@ int gl_mm_sync_bits_to_ghosts(gl_mm_t*, void* stream, uint32_t* bitmap);
 /* cuda::Communicator::Sum/Min/Max on one host scalar
  * (grape/cuda/communication/communicator.h:41-84,160-172): device-side peer
  * all-reduce, bit-identical on every rank (fixed fid order).
- * dtype: 0 int64, 1 double; op: 0 sum, 1 min, 2 max.  Synchronises `stream`. */
+ * dtype: 0 int64, 1 double; op: 0 sum, 1 min, 2 max.  Synchronises `stream`.
+ * The result is the left fold in fid order (sum: ((v0 + v1) + v2) ...); min / max
+ * keep the running value only when it compares strictly less / greater, so of
+ * values that compare equal (-0.0 and +0.0) the one of the highest fid wins. */
 int gl_allreduce(gl_mm_t*, void* stream, void* inout_host, int dtype, int op);
 
 /* ------------------------------------------------------------------ *
@@ -481,9 +485,11 @@ void gl_app_destroy(gl_app_t*);
  * ------------------------------------------------------------------ */
 typedef enum {
   GL_OP_BFS_LEVEL = 0,    /* if level[v]==INF: level[v]=depth; out.insert(v)  */
-  GL_OP_MIN_RELAX_U32 = 1,/* atomicMin(state[v], state[u] (+w))               */
-  GL_OP_MIN_RELAX_F32 = 2,
-  GL_OP_ADD_SCATTER_F64 = 3,
+  GL_OP_MIN_RELAX_U32 = 1,/* atomicMin(state[v], state[u] (+w)); the sum saturates
+                             at 0xFFFFFFFF (unreached), so an unreached source
+                             never relaxes anything                           */
+  GL_OP_MIN_RELAX_F32 = 2,/* as U32 on non-negative floats; unreached = FLT_MAX */
+  GL_OP_ADD_SCATTER_F64 = 3,/* atomicAdd(state2[v], state[u])                 */
   GL_OP_COUNT = 4         /* counts scanned entries only (bandwidth probe)    */
 } gl_edge_op_kind;
 
@@ -493,11 +499,14 @@ typedef struct {
   void* state2;           /* ADD_SCATTER: destination array                    */
   uint32_t* out_bitmap;   /* updated vertices (atomicOr), may be NULL          */
   uint32_t depth;         /* BFS_LEVEL: level to write                         */
-  int use_weight;
+  int use_weight;         /* MIN_RELAX_*: 1 = add the edge's f32 weight (a
+                             fragment without edge data adds 0); a fragment with
+                             f64 edge data is refused with GL_ERR_ARG           */
 } gl_edge_op;
 
 /* ForEachOutgoingEdge(stream, frag, WorkSourceArray(queue,n), op, lb)
- * (parallel_engine.h:987-1013).  queue: device array of n lids. */
+ * (parallel_engine.h:987-1013).  queue: device array of n lids, in any order;
+ * an entry that repeats is scanned once per copy.  Directed fragments scan oe. */
 int gl_edge_scan_queue(const gl_frag_t*, void* stream, const uint32_t* queue,
                        uint32_t n, const gl_edge_op* op, int lb,
                        uint64_t* entries_scanned_host /* may be NULL */);

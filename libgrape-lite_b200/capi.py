@@ -420,6 +420,19 @@ class MessageManager:
         check(lib().gl_mm_send_outer(self.h, None, frag.h, remote_bitmap.ptr,
                                      state.ptr if state is not None else None, int(value_bytes), int(clear_bits)))
 
+    def mirror_plan(self, frag):
+        """gl_mm_mirror_plan: collective, once per (manager, fragment)."""
+        check(lib().gl_mm_mirror_plan(self.h, None, frag.h))
+
+    def sync_values(self, values, elem_bytes):
+        """gl_mm_sync_values_to_ghosts: every outer copy in `values` (device array over
+        inner then outer vertices) takes its owner's value.  Collective."""
+        check(lib().gl_mm_sync_values_to_ghosts(self.h, None, values.ptr, int(elem_bytes)))
+
+    def sync_bits(self, bitmap):
+        """gl_mm_sync_bits_to_ghosts: ghost bits |= owner bits.  Collective."""
+        check(lib().gl_mm_sync_bits_to_ghosts(self.h, None, C.cast(bitmap.ptr, C.POINTER(C.c_uint32))))
+
     def allreduce(self, value, is_double=False, op=0):
         v = C.c_double(value) if is_double else C.c_int64(int(value))
         check(lib().gl_allreduce(self.h, None, C.byref(v), 1 if is_double else 0, int(op)))

@@ -466,6 +466,8 @@ int MessageManager::Init(gl_comm* c, const gl_frag_view& fv, uint32_t item_bytes
   }
   GL_CUDA(d_send_count.alloc(fnum));
   GL_CUDA(cudaMemset(d_send_count, 0, sizeof(uint32_t) * fnum));
+  GL_CUDA(d_zero_count.alloc(fnum));
+  GL_CUDA(cudaMemset(d_zero_count, 0, sizeof(uint32_t) * fnum));
   GL_CUDA(h_send_count.alloc(fnum + 1));
   GL_CUDA(h_result.alloc(1));
   for (int par = 0; par < 2; ++par) {
@@ -510,7 +512,10 @@ MsgView MessageManager::view() const {
     v.send_slot = d_send_slot[par];
     v.send_count = d_send_count;
     v.recv_slot = d_recv_slot[prev];
-    v.recv_count = (const uint32_t*) comm->local_base + (size_t) prev * GL_MAX_FNUM;
+    // round 0 of a query receives nothing: the parity-1 count cells still hold a round of the
+    // previous query on this manager
+    v.recv_count = round == 0 ? d_zero_count.get()
+                              : (const uint32_t*) comm->local_base + (size_t) prev * GL_MAX_FNUM;
   }
   return v;
 }

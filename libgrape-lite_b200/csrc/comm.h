@@ -100,6 +100,7 @@ struct MessageManager {
   DevBuf<char*> d_send_slot[2];          // [parity][fnum]
   DevBuf<const char*> d_recv_slot[2];    // [parity][fnum]
   DevBuf<uint32_t> d_send_count;         // [fnum]
+  DevBuf<uint32_t> d_zero_count;         // [fnum] zeros: what round 0 of a query receives
   PinnedBuf<uint32_t> h_send_count;      // [fnum+1]
   DevBuf<uint32_t*> d_peer_count[2];     // [parity][fnum] address of my count cell at peer
 

@@ -199,9 +199,27 @@ GL_DEV bool next_super_tile(SM& sm, unsigned int* ticket, uint32_t nverts,
   }
 }
 
+// The hub list is sized for a frontier, where a row appears once.  A queue may repeat an entry
+// (ForEach over an array processes every entry), so a queue of copies of one long row can emit
+// more work items than the list holds.  Ops that can be handed such a queue declare
+// `static constexpr bool kHubOverflowInline = true`: the entries of the items past hub_cap are
+// then walked where the row was met instead of being dropped.  Everybody else compiles to
+// exactly the same code as before.
+template <class Op, class = void>
+struct op_hub_overflow_inline : std::false_type {};
+template <class Op>
+struct op_hub_overflow_inline<Op, std::void_t<decltype(Op::kHubOverflowInline)>>
+    : std::integral_constant<bool, Op::kHubOverflowInline> {};
+
+// first entry of row [b, e) that did not fit into the hub list (e if all of it did)
+GL_DEV uint64_t hub_overflow_begin(uint64_t b, uint64_t e, uint32_t at, uint32_t pieces, uint32_t hub_cap) {
+  if ((uint64_t) at + pieces <= hub_cap) return e;
+  return b + (uint64_t) (at < hub_cap ? hub_cap - at : 0) * kHubChunk;
+}
+
 template <class Op>
 GL_DEV void hub_push(uint32_t v, uint64_t b, uint64_t e, ScanCtrl* ctrl,
-                     HubItem* hubs, uint32_t hub_cap) {
+                     HubItem* hubs, uint32_t hub_cap, EdgeRange er, const Op& op, ScanAcc& acc) {
   const uint64_t dg = e - b;
   uint32_t pieces = (uint32_t) ((dg + kHubChunk - 1) / kHubChunk);
   uint32_t at = atomicAdd(&ctrl->hub_count, pieces);
@@ -213,6 +231,18 @@ GL_DEV void hub_push(uint32_t v, uint64_t b, uint64_t e, ScanCtrl* ctrl,
       h.begin = b + (uint64_t) p * kHubChunk;
       h.end = (h.begin + kHubChunk < e) ? h.begin + kHubChunk : e;
       hubs[at + p] = h;
+    }
+  }
+  if constexpr (op_hub_overflow_inline<Op>::value) {
+    using W = typename Op::W;
+    const uint64_t ob = hub_overflow_begin(b, e, at, pieces, hub_cap);
+    if (ob < e) {  // this thread alone met the row: walk the rest serially
+      const auto meta = op.assign(v);
+      for (uint64_t p = ob; p < e; ++p) {
+        W w = Op::kWeighted ? load_w<W>(er.w, p) : (W) 1;
+        call_edge(op, v, meta, er.col[p], w, p, acc);
+      }
+      atomicAdd(&ctrl->scanned, (unsigned long long) (e - ob));
     }
   }
 }
@@ -242,7 +272,7 @@ GL_DEV void walk_tile(ScanSmem<typename Op::Meta>& sm, uint32_t nf, EdgeRange er
         // source hub costs tens of microseconds)
         uint32_t slot = atomicAdd(&sm.hubn, 1u);
         if (slot < (uint32_t) kMaxTileHubs) sm.hubidx[slot] = i;
-        else hub_push<Op>(v, b, e, ctrl, hubs, hub_cap);
+        else hub_push<Op>(v, b, e, ctrl, hubs, hub_cap, er, op, acc);
         dg = 0;
       }
       degs[k] = (uint32_t) dg;
@@ -279,6 +309,18 @@ GL_DEV void walk_tile(ScanSmem<typename Op::Meta>& sm, uint32_t nf, EdgeRange er
           it.begin = b + (uint64_t) p * kHubChunk;
           it.end = (it.begin + kHubChunk < e) ? it.begin + kHubChunk : e;
           hubs[at + p] = it;
+        }
+      }
+      if constexpr (op_hub_overflow_inline<Op>::value) {
+        using W = typename Op::W;
+        const uint64_t ob = hub_overflow_begin(b, e, at, pieces, hub_cap);
+        if (ob < e) {  // uniform: the CTA walks the entries that did not fit
+          const auto meta = sm.meta[i];
+          for (uint64_t p = ob + threadIdx.x; p < e; p += kTB) {
+            W w = Op::kWeighted ? load_w<W>(er.w, p) : (W) 1;
+            call_edge(op, v, meta, ld_stream_u32(er.col + p), w, p, acc);
+          }
+          if (threadIdx.x == 0) scanned += e - ob;
         }
       }
       __syncthreads();

@@ -9,7 +9,15 @@
 namespace gl {
 namespace {
 
+// Long-row cut of the cm / cmold queue scans: rows longer than this go to the hub phase (cta
+// uses kHubDeg).  A row that long would serialise one CTA: measured 2x slower than the
+// reference's cm.
+constexpr uint32_t kHubDegCm = 8 * kHubDeg;
+
+// Every op below may be handed a queue with repeated entries (see op_hub_overflow_inline).
+
 struct OpLevel {
+  static constexpr bool kHubOverflowInline = true;
   using Meta = uint32_t;
   using W = float;
   static constexpr bool kWeighted = false;
@@ -27,6 +35,7 @@ struct OpLevel {
   }
 };
 struct OpMinU32 {
+  static constexpr bool kHubOverflowInline = true;
   using Meta = uint32_t;
   using W = float;
   static constexpr bool kWeighted = true;
@@ -35,7 +44,12 @@ struct OpMinU32 {
   int use_w;
   GL_DEV Meta assign(uint32_t u) const { return state[u]; }
   GL_DEV void edge(uint32_t, Meta m, uint32_t v, W w, ScanAcc& acc) const {
-    uint32_t nv = use_w ? m + (uint32_t) w : m;
+    // saturating: an unreached source (kInfU32) never relaxes anything
+    uint32_t nv = m;
+    if (use_w) {
+      nv = m + (uint32_t) w;
+      if (nv < m) nv = kInfU32;
+    }
     if (nv < atomicMin(state + v, nv)) {
       if (out) bit_set_atomic(out, v);
       acc.next_count++;
@@ -43,6 +57,7 @@ struct OpMinU32 {
   }
 };
 struct OpMinF32 {
+  static constexpr bool kHubOverflowInline = true;
   using Meta = float;
   using W = float;
   static constexpr bool kWeighted = true;
@@ -59,6 +74,7 @@ struct OpMinF32 {
   }
 };
 struct OpAddF64 {
+  static constexpr bool kHubOverflowInline = true;
   using Meta = double;
   using W = float;
   static constexpr bool kWeighted = false;
@@ -70,6 +86,7 @@ struct OpAddF64 {
   }
 };
 struct OpCount {
+  static constexpr bool kHubOverflowInline = true;
   using Meta = uint32_t;
   using W = float;
   static constexpr bool kWeighted = false;
@@ -144,9 +161,8 @@ int scan_queue(const gl_frag* f, cudaStream_t s, const uint32_t* q, uint32_t n,
       case GL_LB_CM:
       case GL_LB_CMOLD:
       case GL_LB_CTA: {
-        // CTA tiles; rows longer than hub_deg are cut into grid-wide 1024-entry work items (cta: 1024,
-        // cm: 8192 -- a row that long would serialise one CTA: measured 2x slower than the reference's cm)
-        uint32_t hub_deg = lb == GL_LB_CTA ? kHubDeg : 8 * kHubDeg;
+        // CTA tiles; rows longer than hub_deg are cut into grid-wide kHubChunk-entry work items
+        uint32_t hub_deg = lb == GL_LB_CTA ? kHubDeg : kHubDegCm;
         int g = std::min<int>(persistent_grid(k_queue_scan_cta<Op>, di->sm_count), (int) ((n + kTileV - 1) / kTileV));
         GL_LAUNCH(k_queue_scan_cta<Op>, g, kTB, s, ArraySrc{q}, n, er, op, ps.ctrl, ps.hubs, ps.hub_cap, hub_deg);
         int g2 = persistent_grid(k_hub_scan_tma<Op>, di->sm_count);
@@ -200,6 +216,12 @@ int gl_edge_scan_queue(const gl_frag_t* f, void* stream, const uint32_t* queue,
     set_error("fragment topology is offloaded");
     return GL_ERR_STATE;
   }
+  if ((op->kind == GL_OP_MIN_RELAX_U32 || op->kind == GL_OP_MIN_RELAX_F32) && op->use_weight && f->oe.w &&
+      f->edata_bytes != 4) {
+    set_error("gl_edge_scan_queue: use_weight needs f32 edge data (this fragment has %d-byte edge data)",
+              f->edata_bytes);
+    return GL_ERR_ARG;
+  }
   cudaStream_t s = (cudaStream_t) stream;
   switch (op->kind) {
     case GL_OP_BFS_LEVEL: {
@@ -209,12 +231,12 @@ int gl_edge_scan_queue(const gl_frag_t* f, void* stream, const uint32_t* queue,
     }
     case GL_OP_MIN_RELAX_U32: {
       GL_ARG(op->state, "state required");
-      OpMinU32 o{(uint32_t*) op->state, op->out_bitmap, op->use_weight && f->oe.w && f->edata_bytes == 4};
+      OpMinU32 o{(uint32_t*) op->state, op->out_bitmap, op->use_weight && f->oe.w != nullptr};
       return scan_queue(f, s, queue, n, o, lb, entries_scanned_host);
     }
     case GL_OP_MIN_RELAX_F32: {
       GL_ARG(op->state, "state required");
-      OpMinF32 o{(float*) op->state, op->out_bitmap, op->use_weight && f->oe.w && f->edata_bytes == 4};
+      OpMinF32 o{(float*) op->state, op->out_bitmap, op->use_weight && f->oe.w != nullptr};
       return scan_queue(f, s, queue, n, o, lb, entries_scanned_host);
     }
     case GL_OP_ADD_SCATTER_F64: {

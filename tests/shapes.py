@@ -13,6 +13,8 @@ are exact in f32 and f64 alike.
 import numpy as np
 
 K_HUB_DEG = 1024           # engine.cuh kHubDeg: rows longer than this go to the hub phase
+K_HUB_DEG_CM = 8192        # primitives.cu kHubDegCm: the long-row cut of the queue scan's cm / cmold modes
+K_HUB_CHUNK = 1024         # engine.cuh kHubChunk: entries per hub work item
 K_TILE_V = 1024            # engine.cuh kTileV: vertices per frontier tile
 K_MAX_TILE_HUBS = 32       # engine.cuh kMaxTileHubs: long rows a tile emits cooperatively
 K_DENSE_TILE = 4096        # dense.cuh kDenseTile: CSR entries per dense-sweep tile
@@ -48,18 +50,19 @@ def star(k, centre_last=False):
     return _out(n, np.full(k, c), np.delete(np.arange(n), c))
 
 
-def hub_block(h, base=K_TILE_V + 3, pool=1200):
+def hub_block(h, base=K_TILE_V + 3, pool=1200, cut=K_HUB_DEG):
     """h consecutive ids base..base+h-1 inside one K_TILE_V-aligned block, hub i
-    with the odd degree K_HUB_DEG + 1 + 2i into a shared pool of vertices after
+    with the odd degree cut + 1 + 2i into a shared pool of vertices after
     the block.  h > K_MAX_TILE_HUBS overflows the per-tile hub slots (the
     single-thread hub_push fallback), and the odd degrees make the hub rows --
-    and so their work items -- start at offsets that are not multiples of 4."""
+    and so their work items -- start at offsets that are not multiples of 4.
+    cut = K_HUB_DEG_CM puts the rows over the cut of the queue scan's cm mode."""
     assert base // K_TILE_V == (base + h - 1) // K_TILE_V, "hubs must share one tile"
     pool0 = (base // K_TILE_V + 1) * K_TILE_V
     n = pool0 + pool
     s, d = [], []
     for i in range(h):
-        deg = K_HUB_DEG + 1 + 2 * i
+        deg = cut + 1 + 2 * i
         s.append(np.full(deg, base + i))
         d.append(pool0 + (np.arange(deg) * (i + 1) + i) % pool)   # repeats within a row when deg > pool
     return _out(n, np.concatenate(s), np.concatenate(d))
@@ -139,6 +142,31 @@ def source_heavy(k):
     return _out(k + 1, np.zeros(k), np.arange(1, k + 1))
 
 
+def rows_of_degree(degs, pool=600):
+    """Row i has degs[i] entries into a pool of `pool` vertices after the rows
+    (cycling, so a row longer than the pool repeats neighbours).  Degrees on both
+    sides of a cut (K_HUB_DEG, K_HUB_DEG + 1, K_HUB_DEG_CM, K_HUB_DEG_CM + 1) put
+    rows exactly on it; odd degrees before them shift the next row's first entry
+    off a multiple of 4."""
+    r = len(degs)
+    s = [np.full(d, i) for i, d in enumerate(degs)]
+    d = [r + (np.arange(k) + 7 * i) % pool for i, k in enumerate(degs)]
+    return _out(r + pool, np.concatenate(s), np.concatenate(d))
+
+
+def bipartite_cover(shape, directed=False):
+    """Bipartite double cover: vertex u becomes 2u (side A) and 2u + 1 (side B),
+    and every edge u - v becomes 2u - 2v+1 and 2v - 2u+1 (directed: u -> v
+    becomes 2u -> 2v+1 only).  Row 2u has the degree (out-degree) of row u, and
+    every row of side A points into side B: a queue drawn from side A never
+    changes its own sources, so one relaxation step over it is exactly the
+    Jacobi step in any order."""
+    n, src, dst, w = shape
+    if directed:
+        return 2 * n, 2 * src, 2 * dst + 1, w
+    return 2 * n, np.concatenate([2 * src, 2 * dst]), np.concatenate([2 * dst + 1, 2 * src + 1]), np.concatenate([w, w])
+
+
 def union(shapes, seed=None):
     """Disjoint union with contiguous id ranges, or (seed given) with the ids
     shuffled by a seeded permutation."""
@@ -188,3 +216,82 @@ def hub_rows_unaligned(rp, cut=K_HUB_DEG):
     rp = np.asarray(rp, dtype=np.int64)
     deg = np.diff(rp)
     return int(np.sum((deg > cut) & (rp[:-1] % 4 != 0)))
+
+
+# Path-taken checks of the queue scan (gl_edge_scan_queue, modes cta / cm / cmold): a CTA
+# takes K_TILE_V consecutive queue entries; a row longer than the cut becomes ceil(deg /
+# K_HUB_CHUNK) hub work items, counted once per queue entry.
+def hub_cap(m):
+    """Hub work items the queue scan has room for on a fragment of m CSR entries
+    (primitives.cu ensure_scratch: m / kHubChunk + m / kHubDeg + 1024)."""
+    m = max(int(m), 1)
+    return m // K_HUB_CHUNK + m // K_HUB_DEG + 1024
+
+
+def queue_hub_pieces(rp, q, cut):
+    """Hub work items a queue emits: pieces of every long row, per entry."""
+    rp = np.asarray(rp, dtype=np.int64)
+    deg = (rp[1:] - rp[:-1])[np.asarray(q, dtype=np.int64)]
+    return int(np.sum(np.where(deg > cut, (deg + K_HUB_CHUNK - 1) // K_HUB_CHUNK, 0)))
+
+
+def long_rows_per_queue_tile(rp, q, cut):
+    """Most queue entries with a row longer than `cut` in one K_TILE_V-entry queue tile."""
+    rp = np.asarray(rp, dtype=np.int64)
+    deg = (rp[1:] - rp[:-1])[np.asarray(q, dtype=np.int64)]
+    pos = np.flatnonzero(deg > cut)
+    return 0 if len(pos) == 0 else int(np.bincount(pos // K_TILE_V).max())
+
+
+ROW_DEGREES = [3, K_HUB_DEG, K_HUB_DEG + 1, 1, K_HUB_DEG_CM, K_HUB_DEG_CM + 1, 5, K_HUB_DEG + 1, K_HUB_DEG_CM + 1]
+
+# The graphs of the engine-primitive tests (tests/test_gpu_engine.py), all bipartite covers so that
+# one relaxation step over a side-A queue is exact.  "degrees" is padded with isolated vertices:
+# rows of degree 0.
+ENGINE_SHAPES = {
+    "star": lambda: bipartite_cover(star(70000)),
+    "hub_block": lambda: bipartite_cover(hub_block(33)),
+    "hub_block_cm": lambda: bipartite_cover(hub_block(33, cut=K_HUB_DEG_CM)),
+    "multi_loop": lambda: bipartite_cover(multi_loop()),
+    "degrees": lambda: bipartite_cover(pad_to(rows_of_degree(ROW_DEGREES), len(ROW_DEGREES) + 600 + 40)),
+}
+
+
+def engine_path_checks(name, rp, side_a):
+    """(branch, reached) pairs for the engine-primitive case `name`: on CSR rp,
+    the sorted side-A queue `side_a` -- or 32 copies of its longest row -- takes
+    the queue scan through the branch."""
+    rp = np.asarray(rp, dtype=np.int64)
+    side_a = np.asarray(side_a, dtype=np.int64)
+    deg = rp[1:] - rp[:-1]
+    out = []
+    if name == "star":
+        q = np.full(32, side_a[np.argmax(deg[side_a])])
+        for cut in (K_HUB_DEG, K_HUB_DEG_CM):
+            out.append(("32 copies of the centre: hub items above hub_cap at cut %d" % cut,
+                        queue_hub_pieces(rp, q, cut) > hub_cap(rp[-1])))
+    if name in ("hub_block", "hub_block_cm"):
+        cut = K_HUB_DEG if name == "hub_block" else K_HUB_DEG_CM
+        out.append(("more than %d long rows in one queue tile at cut %d" % (K_MAX_TILE_HUBS, cut),
+                    long_rows_per_queue_tile(rp, side_a, cut) > K_MAX_TILE_HUBS))
+        out.append(("long rows starting off a 4-aligned entry at cut %d" % cut,
+                    queue_hub_rows_unaligned(rp, side_a, cut) > 0))
+    if name == "multi_loop":
+        out.append(("the 5000-fold multi-edge is one long row", deg[side_a].max() > 5000))
+    if name == "degrees":
+        for d in (K_HUB_DEG, K_HUB_DEG + 1, K_HUB_DEG_CM, K_HUB_DEG_CM + 1, 0):
+            out.append(("a row of degree %d" % d, bool(np.any(deg[side_a] == d))))
+        for cut in (K_HUB_DEG, K_HUB_DEG_CM):
+            out.append(("long rows starting off a 4-aligned entry at cut %d" % cut,
+                        queue_hub_rows_unaligned(rp, side_a, cut) > 0))
+    return out
+
+
+def queue_hub_rows_unaligned(rp, q, cut):
+    """Queue entries with a row longer than `cut` whose first entry is not
+    4-aligned: their hub items make the TMA hub phase copy from the enclosing
+    16-byte boundary."""
+    rp = np.asarray(rp, dtype=np.int64)
+    q = np.asarray(q, dtype=np.int64)
+    deg = rp[q + 1] - rp[q]
+    return int(np.sum((deg > cut) & (rp[q] % 4 != 0)))

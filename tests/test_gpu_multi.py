@@ -72,3 +72,24 @@ def test_multi_fragment_shapes_one_device(nproc):
     sys.stdout.write(p.stdout[-4000:])
     assert p.returncode == 0, p.stdout[-4000:]
     assert p.stdout.count(" OK") == 60, p.stdout[-4000:]     # 6 shapes x 10 app configurations
+
+
+@pytest.mark.parametrize("nproc", [2, 3])
+def test_message_manager_face2_one_device(nproc):
+    """The message manager of the C ABI on 2 and 3 fragments of one device, item by item
+    (mgpu_worker.py GL_FACE2=1): send_outer + process for every value size, clear_bits and
+    consumer kind, the round protocol and its termination vote, round 0 of a second query,
+    the dense mirror sync of values and bits, gl_allreduce and a landing-slot overflow -- on
+    a star whose centre has copies on every peer, a path with owner boundaries inside a
+    bitmap word (alone and padded with isolated vertices), fragments without outer vertices
+    and R-MAT 12."""
+    if _ngpus() < 1:
+        pytest.skip("needs a GPU")
+    env = dict(os.environ, GL_ONE_DEVICE="1", GL_FACE2="1")
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", str(nproc),
+           "--master-addr", "127.0.0.1", "--master-port", str(29580 + nproc),
+           os.path.join(ROOT, "tests", "mgpu_worker.py")]
+    p = subprocess.run(cmd, cwd=ROOT, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=900)
+    sys.stdout.write(p.stdout[-6000:])
+    assert p.returncode == 0, p.stdout[-6000:]
+    assert p.stdout.count(" OK") == 5, p.stdout[-6000:]      # 5 graphs

@@ -22,19 +22,29 @@ def graph(shape, directed=False):
     return pyoracle.Graph(n, src, dst, w, directed=directed)
 
 
-def _constexpr(fname, name):
+def _constexpr(fname, name, names=None):
+    """Value of `constexpr T name = expr;` in csrc/fname; expr may use the constants in `names`."""
     text = open(os.path.join(CSRC, fname)).read()
     m = re.search(r"constexpr\s+[\w:]+\s+%s\s*=\s*([^;]+);" % name, text)
     assert m, "%s not found in %s" % (name, fname)
-    return int(eval(m.group(1).replace("u", ""), {}))
+    return int(eval(re.sub(r"(\d)u\b", r"\1", m.group(1)), dict(names or {})))
 
 
 @pytest.mark.parametrize("fname,name,value", [
     ("engine.cuh", "kHubDeg", S.K_HUB_DEG), ("engine.cuh", "kTileV", S.K_TILE_V),
-    ("engine.cuh", "kMaxTileHubs", S.K_MAX_TILE_HUBS), ("dense.cuh", "kDenseTile", S.K_DENSE_TILE),
+    ("engine.cuh", "kMaxTileHubs", S.K_MAX_TILE_HUBS), ("engine.cuh", "kHubChunk", S.K_HUB_CHUNK),
+    ("dense.cuh", "kDenseTile", S.K_DENSE_TILE),
     ("dense.cuh", "kDenseRows", S.K_DENSE_ROWS), ("app_pagerank.cu", "kPrHub", S.K_PR_HUB)])
 def test_shape_constants_match_kernels(fname, name, value):
     assert _constexpr(fname, name) == value
+
+
+def test_queue_scan_cm_cut_matches_kernel():
+    """The cm / cmold cut of gl_edge_scan_queue, and the hub-list size it is checked against."""
+    hub_deg = _constexpr("engine.cuh", "kHubDeg")
+    assert _constexpr("primitives.cu", "kHubDegCm", {"kHubDeg": hub_deg}) == S.K_HUB_DEG_CM
+    text = open(os.path.join(CSRC, "primitives.cu")).read()
+    assert "m / kHubChunk + m / kHubDeg + 1024" in text      # S.hub_cap
 
 
 def test_bfs_thresholds_match_kernel():
@@ -189,3 +199,27 @@ def test_shape_geometry():
     rp = graph(S.multi_loop()).csr()[0]
     assert np.diff(rp.astype(np.int64)).max() > S.K_HUB_DEG
     assert S.max_dense_tile_rows(graph(S.star(1023)).csr()[0]) <= S.K_DENSE_ROWS + 1
+
+
+@pytest.mark.parametrize("name", sorted(S.ENGINE_SHAPES))
+def test_engine_shape_paths(name):
+    """The engine-primitive graphs are bipartite covers whose side-A queues reach
+    the queue scan's branches (long rows over each cut, more than kMaxTileHubs of
+    them in one tile, hub items off a 4-aligned entry, hub items above hub_cap)."""
+    n, src, dst, w = S.ENGINE_SHAPES[name]()
+    rp, col, _ = graph((n, src, dst, w)).csr()
+    side_a = np.arange(0, n, 2)
+    starts = rp[side_a].astype(np.int64)
+    deg = (rp[side_a + 1] - rp[side_a]).astype(np.int64)
+    ent = np.repeat(starts - np.concatenate([[0], np.cumsum(deg)[:-1]]), deg) + np.arange(deg.sum())
+    assert np.all(col[ent] % 2 == 1)                          # side A points into side B only
+    checks = S.engine_path_checks(name, rp, side_a)
+    assert checks and all(ok for _, ok in checks), [what for what, ok in checks if not ok]
+
+
+def test_bipartite_cover_degrees():
+    n, src, dst, w = S.bipartite_cover(S.rows_of_degree(S.ROW_DEGREES))
+    rp = graph((n, src, dst, w)).csr()[0].astype(np.int64)
+    assert list(np.diff(rp)[0:2 * len(S.ROW_DEGREES):2]) == S.ROW_DEGREES
+    nd, sd, dd, wd = S.bipartite_cover(S.path(5), directed=True)
+    assert nd == 10 and list(sd) == [0, 2, 4, 6] and list(dd) == [3, 5, 7, 9]
