@@ -400,10 +400,33 @@ typedef enum {
    * (a multi-edge counts once per copy, a self loop twice) */
   GL_APP_CORE_DECOMPOSITION = 7, /* core_decomposition/core_decomposition.h
                                     result: int64 core number (isolated: 0)     */
-  GL_APP_KCORE = 8     /* kcore/kcore.h  result: int64 entries whose other
+  GL_APP_KCORE = 8,    /* kcore/kcore.h  result: int64 entries whose other
                           endpoint survives the k-core peel (k = max_round);
                           v is in the k-core iff value >= k                   */
+  GL_APP_KCLIQUE = 9   /* kclique/kclique.h (--kclique_k = max_round), see below */
 } gl_app_kind;
+
+/* GL_APP_KCLIQUE: k = max_round, 3 <= k <= GL_KCLIQUE_MAX_K; a smaller or larger k and a directed
+ * fragment are refused at gl_app_create with GL_ERR_ARG.  The result is ONE int64 (gl_app_result takes
+ * bytes >= 8): the number of k-cliques of the whole fragment group, the same value on every rank.
+ * Counting is on the simple graph underneath the fragments: self loops are ignored, a pair joined by
+ * several CSR entries is one edge, a k-clique is a set of k distinct pairwise adjacent vertices.  On a
+ * simple graph this is the sum of the reference's per-fragment clique_num at any fragment count.  On a
+ * multigraph it deliberately differs: the reference weights a clique by the multiplicities of some of
+ * its edges, in an order that depends on the fragment count.  The count is accumulated in uint64 and
+ * wraps modulo 2^64 (the reference's size_t); the int64 holds those bits.  One fragment holds at most
+ * 2^32 - 1 oriented edges (edges from one of its vertices to a higher-ranked one).
+ * Stats: supersteps = worker rounds (1); entries_scanned = DAG entries iterated by the intersections;
+ * frontier_vertices = oriented edges of this fragment; step_frontier[0] = the largest candidate set
+ * |N+(u) ∩ N+(v)| of an oriented edge (u, v) of this fragment; step_frontier[1..3] = edges counted by
+ * the warp tier (candidate set <= 32), the CTA bitmap tier (<= 1024) and the CTA list tier (> 1024),
+ * for k >= 4 (0 for k = 3, which sums the candidate set sizes).
+ * GL_KCLIQUE_MAX_K: the depth-first walks keep a stack of max(k - 4, 1) levels of one candidate
+ * bitmap pair per warp in shared memory next to the 128 KB bitmap matrix; at k = 32 a CTA uses
+ * 188 KB of the 227 KB a Hopper CTA can opt into.
+ * Several fragments: a fragment with 2^32 or more oriented edges makes every rank's query return
+ * GL_ERR_ARG. */
+#define GL_KCLIQUE_MAX_K 32
 
 typedef struct {
   int lb;                /* gl_lb (AppConfig::lb, cuda/app_config.h:22-27)     */

@@ -10,9 +10,9 @@ LIB_PATH = os.path.join(_HERE, "libgrape_b200.so")
 
 GL_LB = {"none": 0, "cm": 1, "wm": 2, "cta": 3, "strict": 4, "cmold": 5}
 APP = {"bfs": 0, "sssp": 1, "wcc": 2, "pagerank": 3, "cdlp": 4, "lcc": 5, "wcc_opt": 6,
-       "core_decomposition": 7, "kcore": 8}
+       "core_decomposition": 7, "kcore": 8, "kclique": 9}
 RESULT_DTYPE = {0: np.int64, 1: np.float64, 2: np.int64, 3: np.float64, 4: np.int64, 5: np.float64, 6: np.int64,
-                7: np.int64, 8: np.int64}
+                7: np.int64, 8: np.int64, 9: np.int64}
 GL_MAX_STEP_STATS = 512
 GL_IPC_HANDLE_BYTES = 64
 
@@ -451,15 +451,18 @@ def bitmap_count(bitmap_dev, nbits):
 
 
 class App:
-    """One PIE app bound to a fragment (GPUWorker analogue).  "kcore" takes its
-    k as App("kcore", frag, k=...) (carried in max_round); it has no default."""
+    """One PIE app bound to a fragment (GPUWorker analogue).  "kcore" and "kclique"
+    take their k as App("kcore", frag, k=...) (carried in max_round); it has no
+    default.  The result of "kclique" is one Python int: the k-clique count of the
+    whole fragment group (result() takes no out array for it)."""
 
     def __init__(self, kind, frag, comm=None, **cfg):
         self.kind = APP[kind] if isinstance(kind, str) else kind
         self.frag = frag
-        if self.kind == APP["kcore"]:
+        if self.kind in (APP["kcore"], APP["kclique"]):
             if "k" not in cfg:
-                raise GrapeError("kcore needs k: App('kcore', frag, k=...)")
+                name = "kcore" if self.kind == APP["kcore"] else "kclique"
+                raise GrapeError("%s needs k: App('%s', frag, k=...)" % (name, name))
             cfg["max_round"] = int(cfg.pop("k"))
         c = AppConfig()
         lib().gl_app_config_default(C.byref(c))
@@ -488,6 +491,12 @@ class App:
 
     def result(self, out=None):
         dt = RESULT_DTYPE[self.kind]
+        if self.kind == APP["kclique"]:
+            if out is not None:
+                raise GrapeError("kclique returns one int; result() takes no out array")
+            one = np.zeros(1, dtype=dt)
+            check(lib().gl_app_result(self.h, _p(one), one.nbytes))
+            return int(one.view(np.uint64)[0])   # the uint64 count (modulo 2^64)
         if out is None:
             out = np.empty(self.frag.ivnum, dtype=dt)
         check(lib().gl_app_result(self.h, _p(out), out.nbytes))

@@ -30,6 +30,20 @@ struct Engine {
   int fetch_ctrl();                 // D2H + sync; h_ctrl valid afterwards
 };
 
+// Every fragment's CSR part (row pointers over its inner vertices, m column entries) replicated on every
+// fragment of the group: CUDA IPC export, one blob exchange, bulk peer copies, then a peer barrier so no
+// fragment changes its arrays while a peer still reads them.  Collective when fnum > 1.  The device
+// tables d_rp / d_col [fnum] point at the replicas and, at [fid], at this fragment's own arrays (which
+// must be whole cudaMalloc allocations).
+struct PeerCsr {
+  std::vector<DevBuf<uint64_t>> rep_rp;
+  std::vector<DevBuf<uint32_t>> rep_col;
+  DevBuf<const uint64_t*> d_rp;
+  DevBuf<const uint32_t*> d_col;
+  int replicate(MessageManager& mm, cudaStream_t s, const gl_frag_view& fv, const uint64_t* rp,
+                const uint32_t* col, uint64_t m);
+};
+
 struct StepRecorder {
   std::vector<cudaEvent_t> ev;
   std::vector<uint64_t> entries;
@@ -64,6 +78,7 @@ struct gl_app {
   virtual int IncEval() = 0;
   virtual int Result(void* host_out, size_t bytes) = 0;
   virtual size_t ResultElemBytes() const = 0;
+  virtual size_t ResultCount() const { return frag ? frag->ivnum : 0; }   // elements gl_app_result writes
   virtual void FillStats(gl_query_stats*) {}   // apps that time supersteps on the device
   virtual void AfterRound() {}                 // runs after every FinishARound (global round statistics)
   // Apps whose whole query is one launch record this event in-stream right after the query's last
@@ -99,4 +114,5 @@ gl_app* make_lcc();
 gl_app* make_wcc_opt();
 gl_app* make_core_decomposition();
 gl_app* make_kcore();
+gl_app* make_kclique();
 }  // namespace gl

@@ -124,20 +124,6 @@ k_lcc_tri(const uint64_t* __restrict__ orp, const uint32_t* __restrict__ ocol,
 
 
 // ---------------------------------------------------------------- fnum > 1
-struct GidOf {
-  uint32_t ivnum, fid;
-  int fid_offset;
-  const uint32_t* ovgid;
-  GL_DEV uint32_t operator()(uint32_t x) const {
-    return x < ivnum ? ((fid << fid_offset) | x) : ovgid[x - ivnum];
-  }
-};
-
-__global__ void k_lcc_deg(const uint64_t* __restrict__ rp, uint32_t ivnum, uint32_t* deg) {
-  uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v < ivnum) deg[v] = (uint32_t) (rp[v + 1] - rp[v]);
-}
-
 __global__ void k_lcc_count_m(const uint64_t* __restrict__ rp, const uint32_t* __restrict__ col,
                               const uint32_t* __restrict__ deg, GidOf gid, uint32_t ivnum, uint64_t* cnt) {
   const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
@@ -244,12 +230,6 @@ struct LccApply {
   }
 };
 
-// what a fragment tells its peers about its part of the DAG
-struct LccExport {
-  cudaIpcMemHandle_t h_orp, h_key;
-  uint64_t ivnum, om;
-};
-
 __global__ void k_lcc_out(const uint64_t* rp, const unsigned long long* tri,
                           uint32_t ivnum, double* out) {
   uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
@@ -268,12 +248,7 @@ struct LccApp : gl_app {
   int stage = 0;
   uint32_t tvnum = 0;
   size_t words = 0;
-  // replicas of the peers' DAG parts (fnum > 1; the entry of this fragment stays empty)
-  std::vector<DevBuf<uint64_t>> rep_orp;
-  std::vector<DevBuf<uint32_t>> rep_key;
-  // device tables [fnum] of the DAG parts: the replicas, and orp / ocol at [fid]
-  DevBuf<const uint64_t*> d_t_orp;
-  DevBuf<const uint32_t*> d_t_key;
+  PeerCsr peers;   // fnum > 1: every fragment's part of the DAG
 
   size_t ResultElemBytes() const override { return sizeof(double); }
 
@@ -288,8 +263,6 @@ struct LccApp : gl_app {
     if (fv.fnum > 1) {
       GL_CUDA(deg.alloc(std::max<uint32_t>(tvnum, 1)));
       GL_CUDA(remote.alloc(words));
-      GL_CUDA(d_t_orp.alloc(fv.fnum));
-      GL_CUDA(d_t_key.alloc(fv.fnum));
       GL_TRY(mm.BuildMirrorPlan(eng.stream, fv));
     }
     return GL_OK;
@@ -343,7 +316,7 @@ struct LccApp : gl_app {
     cudaStream_t s = eng.stream;
     const GidOf gid{fv.ivnum, fv.fid, fv.fid_offset, fv.ovgid};
     // 1. degrees: own rows, then the owners' values for the outer copies
-    if (fv.ivnum) GL_LAUNCH(k_lcc_deg, (fv.ivnum + 255) / 256, 256, s, fv.oe_rp, fv.ivnum, deg);
+    if (fv.ivnum) GL_LAUNCH(k_row_length<uint32_t>, (fv.ivnum + 255) / 256, 256, s, fv.oe_rp, fv.ivnum, deg.get());
     GL_TRY(mm.SyncValuesToGhosts(s, deg, 4));
     // 2. my part of the DAG, global ids, rows sorted by gid
     GL_LAUNCH(k_lcc_count_m, eng.sm_count * 8, 256, s, fv.oe_rp, fv.oe_col, deg, gid, fv.ivnum, cnt);
@@ -364,45 +337,8 @@ struct LccApp : gl_app {
                                                   (int64_t) fv.ivnum, orp.get(), orp + 1, s));
       GL_CUDA(cudaStreamSynchronize(s));
     }
-    // 3. export my arrays, replicate the peers' (bulk NVLink copies)
-    LccExport mine;
-    memset(&mine, 0, sizeof(mine));
-    GL_CUDA(cudaIpcGetMemHandle(&mine.h_orp, orp));
-    GL_CUDA(cudaIpcGetMemHandle(&mine.h_key, ocol));
-    mine.ivnum = fv.ivnum;
-    mine.om = om;
-    std::vector<char> all;
-    GL_TRY(mm.ExchangeBlobs(s, &mine, sizeof(mine), &all));
-    rep_orp.clear();
-    rep_key.clear();
-    rep_orp.resize(fv.fnum);
-    rep_key.resize(fv.fnum);
-    std::vector<const uint64_t*> r_orp(fv.fnum);
-    std::vector<const uint32_t*> r_key(fv.fnum);
-    for (uint32_t g = 0; g < fv.fnum; ++g) {
-      if (g == fv.fid) {
-        r_orp[g] = orp;
-        r_key[g] = ocol;
-        continue;
-      }
-      const LccExport& ex = *(const LccExport*) (all.data() + (size_t) g * sizeof(LccExport));
-      GL_CUDA(rep_orp[g].alloc(ex.ivnum + 1));
-      GL_CUDA(rep_key[g].alloc(std::max<uint64_t>(ex.om, 4)));
-      r_orp[g] = rep_orp[g];
-      r_key[g] = rep_key[g];
-      void *p_orp = nullptr, *p_key = nullptr;
-      GL_CUDA(cudaIpcOpenMemHandle(&p_orp, ex.h_orp, cudaIpcMemLazyEnablePeerAccess));
-      GL_CUDA(cudaIpcOpenMemHandle(&p_key, ex.h_key, cudaIpcMemLazyEnablePeerAccess));
-      GL_CUDA(cudaMemcpyAsync(rep_orp[g], p_orp, sizeof(uint64_t) * (ex.ivnum + 1), cudaMemcpyDeviceToDevice, s));
-      if (ex.om) GL_CUDA(cudaMemcpyAsync(rep_key[g], p_key, sizeof(uint32_t) * ex.om, cudaMemcpyDeviceToDevice, s));
-      GL_CUDA(cudaStreamSynchronize(s));
-      GL_CUDA(cudaIpcCloseMemHandle(p_orp));
-      GL_CUDA(cudaIpcCloseMemHandle(p_key));
-    }
-    GL_CUDA(cudaMemcpyAsync(d_t_orp, r_orp.data(), sizeof(void*) * fv.fnum, cudaMemcpyHostToDevice, s));
-    GL_CUDA(cudaMemcpyAsync(d_t_key, r_key.data(), sizeof(void*) * fv.fnum, cudaMemcpyHostToDevice, s));
-    GL_CUDA(cudaStreamSynchronize(s));
-    GL_TRY(mm.PeerBarrier(s));   // every peer has finished reading my arrays
+    // 3. replicate the peers' parts (bulk NVLink copies)
+    GL_TRY(peers.replicate(mm, s, fv, orp, ocol, om));
     mm.ForceContinue();
     return GL_OK;
   }
@@ -417,7 +353,7 @@ struct LccApp : gl_app {
       if (fv.fnum == 1) {
         if (om) GL_LAUNCH(k_lcc_tri, eng.sm_count * 8, 256, s, orp, ocol, osrc, om, tri, eng.ctrl);
       } else {
-        if (om) GL_LAUNCH(k_lcc_tri_m, eng.sm_count * 8, 256, s, orp, ocol, olid, osrc, om, d_t_orp, d_t_key,
+        if (om) GL_LAUNCH(k_lcc_tri_m, eng.sm_count * 8, 256, s, orp, ocol, olid, osrc, om, peers.d_rp, peers.d_col,
                           fv.fid_offset, fv.id_mask, tri, eng.ctrl);
         if (fv.ovnum) GL_LAUNCH(k_lcc_mark_remote, (fv.ovnum + 255) / 256, 256, s, tri, fv.ivnum, fv.ovnum, remote);
         MsgView mv = mm.view();

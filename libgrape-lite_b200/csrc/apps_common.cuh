@@ -177,6 +177,23 @@ k_unpack(MsgView mv, Apply apply, ScanCtrl* ctrl) {
   }
   flush_acc(acc, ctrl);
 }
+
+// lid -> gid of the fragment's vertices (inner: fid << fid_offset | lid; outer: ovgid)
+struct GidOf {
+  uint32_t ivnum, fid;
+  int fid_offset;
+  const uint32_t* ovgid;
+  GL_DEV uint32_t operator()(uint32_t x) const {
+    return x < ivnum ? ((fid << fid_offset) | x) : ovgid[x - ivnum];
+  }
+};
+
+// deg[v] = CSR row length of the inner vertex v (a template so that every app's unit may hold it)
+template <typename T>
+__global__ void k_row_length(const uint64_t* __restrict__ rp, uint32_t ivnum, T* deg) {
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v < ivnum) deg[v] = (T) (rp[v + 1] - rp[v]);
+}
 #endif
 
 // gid-valued label -> oid (WCC / CDLP outputs).  Without a vertex map the

@@ -120,6 +120,7 @@ int gl_app_create(gl_app_t** out, int kind, gl_frag_t* frag, gl_comm_t* comm,
     case GL_APP_WCC_OPT: a = make_wcc_opt(); break;
     case GL_APP_CORE_DECOMPOSITION: a = make_core_decomposition(); break;
     case GL_APP_KCORE: a = make_kcore(); break;
+    case GL_APP_KCLIQUE: a = make_kclique(); break;
     default:
       set_error("unknown app kind %d", kind);
       return GL_ERR_ARG;
@@ -215,7 +216,7 @@ int gl_app_query(gl_app_t* a, gl_query_stats* stats) {
 
 int gl_app_result(gl_app_t* a, void* host_out, size_t bytes) {
   GL_ARG(a && host_out, "null argument");
-  size_t need = a->ResultElemBytes() * (size_t) a->frag->ivnum;
+  size_t need = a->ResultElemBytes() * a->ResultCount();
   if (bytes < need) {
     set_error("result buffer too small: %zu < %zu", bytes, need);
     return GL_ERR_ARG;
