@@ -55,10 +55,22 @@ struct OpBfsPush {
   // the estimate 1.5 * 2^(k-1) is within +-33 %, the switch thresholds are an order-of-magnitude rule.
   const uint8_t* deg8 = nullptr;
   GL_DEV Meta assign(uint32_t) const { return 0; }
+  static GL_DEV unsigned long long degree_of_class(uint32_t k) {
+    return k == 0 ? 0ull : (k == 1 ? 1ull : (3ull << (k - 2)));
+  }
   GL_DEV unsigned long long degree_of(uint32_t v) const {
     if (!deg8) return rp[v + 1] - rp[v];
-    const uint32_t k = deg8[v];
-    return k == 0 ? 0ull : (k == 1 ? 1ull : (3ull << (k - 2)));
+    return degree_of_class(deg8[v]);
+  }
+  // statistics of a vertex this level visited first; `deg` = degree_of(v) when v is inner
+  GL_DEV void note_fresh(uint32_t v, unsigned long long deg, ScanAcc& acc) const {
+    acc.touched++;
+    if (v < ivnum) {
+      acc.next_count++;
+      acc.next_edges += deg;
+    } else {
+      acc.remote++;
+    }
   }
   // Hub rows, 32 consecutive entries per call (engine.cuh, has_warp_entries).  The rows of the
   // hub-first shadow graph are sorted, so neighbouring lanes mostly hit the same bitmap word: the
@@ -66,16 +78,23 @@ struct OpBfsPush {
   // per bitmap instead of one per entry (the source hub of a scale-24 R-MAT graph has 7e5 entries
   // over 2e4 words).  Exactly the per-entry semantics: a bit counts for the first lane of the run
   // that carries it, and only if the word did not hold it before.
+  // Two parts, so that a caller can have the bitmap reads of several calls in flight at once:
+  // warp_edge_bit (load) and warp_edge_set (update).
   static constexpr bool kWarpEntries = true;
   GL_DEV void warp_edge(uint32_t v, bool valid, ScanAcc& acc) const {
+    const uint32_t bit = warp_edge_bit(v, valid);
+    if (!__any_sync(0xffffffffu, bit != 0)) return;
+    if (warp_edge_set(v, bit)) note_fresh(v, v < ivnum ? degree_of(v) : 0ull, acc);
+  }
+  // v's bit unless the visited bitmap already holds it (plain, possibly stale read)
+  GL_DEV uint32_t warp_edge_bit(uint32_t v, bool valid) const {
+    return valid ? (1u << (v & 31)) & ~vis[v >> 5] : 0u;
+  }
+  // All lanes converged.  Sets the lanes' bits in vis / nxt (/ remote); true on the lane whose
+  // entry visited v first.
+  GL_DEV bool warp_edge_set(uint32_t v, uint32_t bit) const {
     const uint32_t lane = lane_id();
     const uint32_t w = v >> 5;
-    uint32_t bit = 0;
-    if (valid) {
-      bit = 1u << (v & 31);
-      bit &= ~vis[w];                    // plain (possibly stale) read first
-    }
-    if (!__any_sync(0xffffffffu, bit != 0)) return;
     // runs of lanes with the same word (invalid / already-visited lanes join their neighbours' runs
     // with an empty bit set, or form runs of their own that end without an atomic)
     const uint32_t wp = __shfl_up_sync(0xffffffffu, w, 1);
@@ -109,15 +128,7 @@ struct OpBfsPush {
     }
     const uint32_t mytail = lane + __ffs(tails >> lane) - 1;
     old = __shfl_sync(0xffffffffu, old, mytail);
-    if (bit & ~old & ~excl) {
-      acc.touched++;
-      if (v < ivnum) {
-        acc.next_count++;
-        acc.next_edges += degree_of(v);
-      } else {
-        acc.remote++;
-      }
-    }
+    return (bit & ~old & ~excl) != 0;
   }
   GL_DEV void edge(uint32_t, Meta, uint32_t v, W, ScanAcc& acc) const {
     if (bit_test(vis, v)) return;        // plain (possibly stale) read first
@@ -658,9 +669,10 @@ struct BfsFusedCtl {
   uint32_t pad;
   unsigned long long src_deg, m_total, touched;
   unsigned long long t_begin;
-  // state the kernel starts from: written by the seed kernel, and by the
-  // kernel itself when it stops because the level-bitmap ring is full (the
-  // host spills the finished levels and relaunches)
+  // state a relaunch starts from: parked by the kernel when it stops because
+  // the level-bitmap ring is full (the host spills the finished levels and
+  // relaunches); several fragments: also the first launch's, from the seed kernel
+  // (k_bfs_fused derives its first launch's state from its arguments)
   unsigned long long r_nf, r_mf, r_visited_edges, r_visited_cnt;
   uint32_t r_phase, r_pad;   // r_phase = ~0: derive from the seed
   unsigned long long p_nf, p_mf, p_visited_edges, p_visited_cnt;   // parked state (-> r_* by k_bfs_resume_prep)
@@ -713,33 +725,12 @@ GL_DEV uint32_t bfs_next_phase(uint32_t phase, unsigned long long n_f,
   return 2u;
 }
 
-// seed_hubs (k_bfs_fused): a source row longer than hub_deg is cut into its hub work items here,
-// by the whole block, so that level 0 is the hub phase alone (no frontier sweep, one grid.sync fewer)
+// first launch of a several-fragment query (k_bfs_fused_multi); k_bfs_fused seeds itself
 __global__ void k_bfs_seed_fused(uint32_t src, int has_src, uint32_t* lv0,
                                  uint32_t* vis, const uint64_t* rp,
-                                 unsigned long long m_total, BfsFusedCtl* ctl,
-                                 int seed_hubs = 0, HubItem* hubs = nullptr, uint32_t hub_cap = 0, uint32_t hub_deg = 0) {
-  if (blockIdx.x != 0) return;
-  uint32_t pieces = 0;
-  if (seed_hubs && has_src) {
-    const uint64_t b = rp[src], e = rp[src + 1];
-    if (e - b > hub_deg) {
-      pieces = (uint32_t) ((e - b + kHubChunk - 1) / kHubChunk);
-      for (uint32_t p = threadIdx.x; p < pieces && p < hub_cap; p += blockDim.x) {
-        HubItem it;
-        it.v = src;
-        it.pad = 0;
-        it.begin = b + (uint64_t) p * kHubChunk;
-        it.end = (it.begin + kHubChunk < e) ? it.begin + kHubChunk : e;
-        hubs[p] = it;
-      }
-    }
-  }
-  if (threadIdx.x != 0) return;
+                                 unsigned long long m_total, BfsFusedCtl* ctl) {
+  if (blockIdx.x != 0 || threadIdx.x != 0) return;
   ctl->c[0] = ScanCtrl();
-  // as the frontier sweep of level 0 would have left them: the source expanded, its row listed
-  ctl->c[0].hub_count = pieces;
-  ctl->c[0].frontier = pieces ? 1 : 0;
   ctl->c[1] = ScanCtrl();
   ctl->c[2] = ScanCtrl();
   ctl->levels = 0;
@@ -816,31 +807,141 @@ struct BfsFusedArgs {
   uint32_t push_v;       // push levels sweep the frontier over lids [0, push_v)
   unsigned long long m_total;   // CSR entries of the graph (the push -> pull rule)
   uint32_t list_gap;             // pull levels try the tail list once at most this many vertices are unvisited
+  uint32_t src;                  // the source's lid (k_bfs_fused, first launch)
+  int has_src;
 };
+
+// Level 0 of a query that starts at a source, pushed: the frontier is the source alone, so the
+// level is its row, split statically over every warp of the grid -- contiguous runs of 32-entry
+// groups aligned to 128 bytes, at most kSrcGroups per warp and pass.  No work list, no ticket and no
+// CTA barrier per item.  A warp issues all its column loads, then all its visited-bitmap reads, then the degree
+// classes of the entries not yet visited (speculatively: deg8 depends on v only), and only then the
+// bit updates group by group, so that the loads' latencies overlap instead of forming one chain per
+// group.  The source counts as visited (thread 0 sets its bit concurrently): its own entries -- self
+// loops -- never count.
+constexpr uint32_t kSrcGroups = 8;
+GL_DEV void bfs_source_row_push(const EdgeRange& er, const OpBfsPush& op, uint32_t src, ScanCtrl* C, ScanAcc& acc) {
+  const uint64_t b = er.rp[src], e = er.rp[src + 1];
+  const uint32_t* row = er.col + (b & ~31ull);   // the row from the start of its first group
+  const uint64_t span = e - (b & ~31ull);
+  const uint32_t ng = (uint32_t) ((span + 31) >> 5);   // the row's 32-entry groups (4-byte entries: < 2^32)
+  const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t wid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const uint32_t per = min((ng + warps - 1) / warps, kSrcGroups);
+  const uint32_t lane = lane_id();
+  for (uint32_t g = wid * per; g < ng; g += warps * per) {
+    // the slice's entries are [lo, hi) from the start of its first group
+    const uint32_t lo = g == 0 ? (uint32_t) b & 31u : 0u;
+    const uint32_t hi = (uint32_t) min(span - ((uint64_t) g << 5), (uint64_t) per * 32);
+    const uint32_t* q = row + ((uint64_t) g << 5) + lane;
+    // (the per-entry state is packed: bit j of `unvis` / byte j of `cls` belong to v[j])
+    uint32_t v[kSrcGroups];
+#pragma unroll
+    for (uint32_t j = 0; j < kSrcGroups; ++j) {
+      const uint32_t o = 32 * j + lane;
+      v[j] = (o >= lo && o < hi) ? ld_stream_u32(q + 32 * j) : src;   // src: no entry
+    }
+    uint32_t unvis = 0;
+#pragma unroll
+    for (uint32_t j = 0; j < kSrcGroups; ++j) unvis |= op.warp_edge_bit(v[j], v[j] != src) ? 1u << j : 0u;
+    uint64_t cls = 0;
+#pragma unroll
+    for (uint32_t j = 0; j < kSrcGroups; ++j)
+      if (((unvis >> j) & 1u) && op.deg8 && v[j] < op.ivnum) cls |= (uint64_t) op.deg8[v[j]] << (8 * j);
+    // group by group: the entry at hand is always v[0] (the array shifts, so it stays in registers)
+#pragma unroll 1
+    for (uint32_t j = 0; j < per; ++j) {
+      const uint32_t bit = (unvis & 1u) << (v[0] & 31);
+      if (__any_sync(0xffffffffu, bit != 0) && op.warp_edge_set(v[0], bit))
+        op.note_fresh(v[0], op.deg8 ? OpBfsPush::degree_of_class((uint32_t) cls & 0xFFu) : op.degree_of(v[0]), acc);
+      unvis >>= 1;
+      cls >>= 8;
+#pragma unroll
+      for (uint32_t k = 0; k + 1 < kSrcGroups; ++k) v[k] = v[k + 1];
+    }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    C->scanned = e - b;
+    C->frontier = 1;
+  }
+}
+
+// flush_acc for a phase after which every warp of the grid holds counts (bfs_source_row_push): the
+// CTA sums them first and adds them with one atomic per counter: with an atomic per warp and
+// counter (flush_acc), level 0 took 7 us longer on an H100 at 700 W.  Leaves `acc` empty.
+struct AccSmem {
+  unsigned long long v[5][kTB / 32];
+};
+GL_DEV void flush_acc_cta(ScanAcc& acc, ScanCtrl* c, AccSmem& sm) {
+  static_assert(offsetof(ScanCtrl, touched) - offsetof(ScanCtrl, next_count) == 4 * sizeof(unsigned long long),
+                "next_count, next_edges, remote_count, aux, touched are consecutive");
+  const uint32_t wid = threadIdx.x >> 5;
+  const unsigned long long s0 = warp_sum((unsigned long long) acc.next_count);
+  const unsigned long long s1 = warp_sum((unsigned long long) acc.next_edges);
+  const unsigned long long s2 = warp_sum((unsigned long long) acc.remote);
+  const unsigned long long s3 = warp_sum((unsigned long long) acc.aux);
+  const unsigned long long s4 = warp_sum((unsigned long long) acc.touched);
+  if (lane_id() == 0) {
+    sm.v[0][wid] = s0;
+    sm.v[1][wid] = s1;
+    sm.v[2][wid] = s2;
+    sm.v[3][wid] = s3;
+    sm.v[4][wid] = s4;
+  }
+  __syncthreads();
+  if (threadIdx.x < 5) {
+    unsigned long long s = 0;
+#pragma unroll
+    for (int w = 0; w < kTB / 32; ++w) s += sm.v[threadIdx.x][w];
+    if (s) atomicAdd(&c->next_count + threadIdx.x, s);
+  }
+  acc = ScanAcc();
+}
 
 // Level d reads lv[d] and writes lv[d+1] (pre-zeroed).  Every thread derives
 // the push/pull decision from the same counters, so nothing is published
 // between levels: one grid.sync per pull level, two per push level (tile
-// phase | hub phase).
+// phase | hub phase) except a first launch's level 0 (bfs_source_row_push).
+// The control block starts zeroed (BfsApp::Init; k_bfs_resume_prep before a
+// relaunch).
 __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedArgs a) {
   cg::grid_group grid = cg::this_grid();
   __shared__ __align__(128) union {
     ScanSmem<uint32_t> scan;
     PullSmem pull;
     HubTmaSmem hub;
+    AccSmem acc;
   } sm;
   __shared__ uint32_t s_item;
   BfsFusedCtl* ctl = a.ctl;
   const uint32_t gtid = blockIdx.x * blockDim.x + threadIdx.x;
   // running totals, replicated in every thread
-  unsigned long long n_f = ctl->r_nf;
-  unsigned long long m_f = ctl->r_mf;
-  unsigned long long visited_edges = ctl->r_visited_edges;
+  unsigned long long n_f, m_f, visited_edges, visited_cnt;
   const unsigned long long m_total = a.m_total;   // a kernel parameter: no register held across the levels
-  unsigned long long visited_cnt = ctl->r_visited_cnt;
-  uint32_t phase = ctl->r_phase;
-  if (phase == 0xFFFFFFFFu)
+  uint32_t phase;
+  if (a.depth_base == 0) {
+    // first launch: the query starts here, with the source as the frontier of level 0
+    const unsigned long long deg = a.has_src ? a.er.rp[a.src + 1] - a.er.rp[a.src] : 0ull;
+    n_f = visited_cnt = a.has_src ? 1ull : 0ull;
+    m_f = visited_edges = deg;
     phase = bfs_next_phase(0, n_f, m_f, m_total - visited_edges, a.pa.ivnum, a.direction_opt, a.beta, a.nz_total);
+    if (gtid == 0) {
+      ctl->t_begin = global_ns();
+      if (a.has_src) {
+        const uint32_t bit = 1u << (a.src & 31);
+        a.lv[a.src >> 5] |= bit;
+        atomicOr(a.vis + (a.src >> 5), bit);   // other warps may set bits of the same word
+      }
+    }
+    // a pull level 0 reads both bitmaps (and owns visited words)
+    if (phase != 0) grid.sync();
+  } else {
+    n_f = ctl->r_nf;
+    m_f = ctl->r_mf;
+    visited_edges = ctl->r_visited_edges;
+    visited_cnt = ctl->r_visited_cnt;
+    phase = ctl->r_phase;
+  }
   for (uint32_t depth = 0; n_f != 0; ++depth) {
     if (depth + 1 >= a.max_lv) {
       // ring full: park the state; the host spills levels [0, max_lv-1) and relaunches (the tail
@@ -873,13 +974,15 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
                                   a.pa.list_cap && a.nz_total <= visited_cnt + a.list_gap);
     } else {
       OpBfsPush op{a.vis, nxt, nullptr, a.er.rp, a.pa.ivnum, a.deg8};
-      // level 0 of a query whose seed listed the source row's hub items: nothing else to sweep for
-      if (depth != 0 || ((const volatile ScanCtrl*) C)->hub_count == 0) {
+      if (depth == 0 && a.depth_base == 0) {
+        bfs_source_row_push(a.er, op, a.src, C, acc);
+        flush_acc_cta(acc, C, sm.acc);
+      } else {
         frontier_scan_phase<OpBfsPush>(sm.scan, cur, a.push_v, a.er, op, C, a.hubs, a.hub_cap, a.hub_deg, acc);
         grid.sync();
+        if (a.hub_tma) hub_scan_phase_tma<OpBfsPush>(sm.hub, a.er, op, C, a.hubs, a.hub_cap, acc);
+        else hub_scan_phase<OpBfsPush>(&s_item, a.er, op, C, a.hubs, a.hub_cap, acc);
       }
-      if (a.hub_tma) hub_scan_phase_tma<OpBfsPush>(sm.hub, a.er, op, C, a.hubs, a.hub_cap, acc);
-      else hub_scan_phase<OpBfsPush>(&s_item, a.er, op, C, a.hubs, a.hub_cap, acc);
     }
     flush_acc(acc, C);
     grid.sync();
@@ -1781,6 +1884,8 @@ struct BfsApp : gl_app {
     depth_base = 0;
     GL_CUDA(cudaMemsetAsync(vis, 0, sizeof(uint32_t) * words, s));
     GL_CUDA(cudaMemsetAsync(remote, 0, sizeof(uint32_t) * words, s));
+    // the fused kernels' level counters and query totals start from zero
+    GL_CUDA(cudaMemsetAsync(d_ctl, 0, sizeof(BfsFusedCtl), s));
     if (global_front && comm->mirror_dirty) {
       // the frontier segments (the first seg_words words of every mirror slot) must be zero when the
       // query starts; the fused kernel leaves them zero, other users of the mirror area do not.
@@ -1840,8 +1945,8 @@ struct BfsApp : gl_app {
     uint32_t src = 0;
     int has_src = has_src_;
     src = src_;   // already translated to the hub-first rank in Setup
-    GL_LAUNCH(k_bfs_seed_fused, 1, 256, s, src, has_src, level_bm(0), vis, g_rp,
-              (unsigned long long) g_m_total, d_ctl, fv.fnum == 1 ? 1 : 0, eng.hubs, eng.hub_cap, eng.hub_deg);
+    const bool multi = fv.fnum > 1;
+    if (multi) GL_LAUNCH(k_bfs_seed_fused, 1, 32, s, src, has_src, level_bm(0), vis, g_rp, (unsigned long long) g_m_total, d_ctl);
     BfsFusedArgs a;
     a.pa = pull_args();
     a.er = EdgeRange{g_rp, g_col, nullptr};
@@ -1861,7 +1966,8 @@ struct BfsApp : gl_app {
     // inside the fused kernel the TMA-staged hub phase is opt-in (GL_HUB_TMA=2); the stand-alone
     // k_hub_scan_tma is the default elsewhere
     a.hub_tma = (getenv("GL_HUB_TMA") && atoi(getenv("GL_HUB_TMA")) == 2) ? 1 : 0;
-    const bool multi = fv.fnum > 1;
+    a.src = src;
+    a.has_src = has_src;
     // one fragment in hub-first order: the vertices with edges are lids [0, nz_total), so the sweeps
     // stop there (a push level also covers an isolated source)
     const bool hub_first = perm && !multi;
@@ -1998,7 +2104,9 @@ struct BfsApp : gl_app {
     int n = (int) std::min<uint32_t>(L + 1, GL_MAX_STEP_STATS);
     st->n_steps = n;
     unsigned long long prev = h_ctl->t_begin;
-    st->step_ms[0] = 0.f;  // PEval (seed) is part of the launch prologue
+    // PEval (seed) is part of the launch prologue.  One fragment: t_begin is the fused kernel's first
+    // instruction, so level 0 does not include the launch; several: the seed kernel's end.
+    st->step_ms[0] = 0.f;
     for (int i = 1; i < n; ++i) {
       const BfsLevelStat& ls = h_ctl->stat[i - 1];
       st->step_ms[i] = (float) ((double) (ls.t_ns - prev) * 1e-6);
