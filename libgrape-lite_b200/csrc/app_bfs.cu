@@ -255,12 +255,11 @@ __global__ void k_bfs_seed(uint32_t src, uint32_t* lv0, uint32_t* vis) {
 // hub_nbr[v] = the inner neighbour of v with the largest out-degree (ties ->
 // first in the row); one warp per row.  Built once per app.
 __global__ void __launch_bounds__(256)
-k_bfs_hub_nbr(const uint64_t* __restrict__ rp, const uint64_t* __restrict__ row_end,
-              const uint32_t* __restrict__ col, uint32_t ivnum, uint32_t* hub_nbr,
+k_bfs_hub_nbr(const uint64_t* __restrict__ rp, const uint32_t* __restrict__ col, uint32_t ivnum, uint32_t* hub_nbr,
               const uint32_t* __restrict__ deg_all = nullptr) {
   const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
   for (uint32_t v = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; v < ivnum; v += warps) {
-    const uint64_t b = rp[v], e = row_end[v];
+    const uint64_t b = rp[v], e = rp[v + 1];
     unsigned long long best = 0;
     for (uint64_t p = b + lane_id(); p < e; p += 32) {
       uint32_t u = col[p];
@@ -305,7 +304,6 @@ struct PullSmem {
 
 struct PullArgs {
   const uint64_t* rp;
-  const uint64_t* row_end;   // end of the inner-neighbour part of each row
   const uint32_t* col;
   const uint32_t* hub_nbr;
   uint32_t ivnum;
@@ -467,7 +465,7 @@ GL_DEV bool bfs_pull_phase(PullSmem& sm, const PullArgs& a,
         uint32_t act = 0, foundm = 0;
 #pragma unroll
         for (int k = 0; k < kIL; ++k) {
-          len[k] = vv[k] != kInfU32 ? (uint32_t) (a.row_end[vv[k]] - bb[k]) : 0u;
+          len[k] = vv[k] != kInfU32 ? (uint32_t) (a.rp[vv[k] + 1] - bb[k]) : 0u;
           if (len[k]) act |= 1u << k;
         }
         for (uint32_t p = 0; p < kPullSerialCap && act; ++p) {
@@ -503,7 +501,7 @@ GL_DEV bool bfs_pull_phase(PullSmem& sm, const PullArgs& a,
       for (uint32_t i = threadIdx.x >> 5; i < nl; i += kTB / 32) {
         const uint32_t v = sm.lng[i];
         const uint64_t b = a.rp[v] + skip;
-        const uint32_t len = (uint32_t) (a.row_end[v] - b);
+        const uint32_t len = (uint32_t) (a.rp[v + 1] - b);
         const uint32_t* row = a.col + b;
         bool hit = false;
         uint32_t p = kPullSerialCap;
@@ -609,7 +607,7 @@ GL_DEV void bfs_list_pull(const PullArgs& a, const uint32_t* __restrict__ cur, u
     if (v != kInfU32) {
       const uint32_t h = a.hub_nbr[v];
       b = a.rp[v] + 1;
-      const uint64_t e = a.row_end[v];
+      const uint64_t e = a.rp[v + 1];
       hit = h != kInfU32 && front_test<false>(a, cur, h);
       len = e > b ? (uint32_t) (e - b) : 0u;
       const uint32_t serial = len < kPullSerialCap ? len : kPullSerialCap;
@@ -667,7 +665,7 @@ struct BfsFusedCtl {
   uint32_t has_src, src_lid;
   uint32_t overflow;   // ran out of level bitmaps
   uint32_t pad;
-  unsigned long long src_deg, m_total, touched;
+  unsigned long long touched;
   unsigned long long t_begin;
   // state a relaunch starts from: parked by the kernel when it stops because
   // the level-bitmap ring is full (the host spills the finished levels and
@@ -683,12 +681,12 @@ struct BfsFusedCtl {
   unsigned long long x_last_tag;
   uint32_t x_msg_rounds, x_mirror_syncs;
   unsigned long long x_items;   // items this GPU sent
-  unsigned long long ph[32][6];
+  unsigned long long ph[32][6];  // GL_TRACE: phase timestamps of the first 32 levels (thread 0)
   unsigned long long xw[32][2];  // GL_TRACE: per level: peer wait / first grid.sync of its last xsync
   unsigned long long l_nf;               // several fragments: this fragment's part of the current frontier (statistics)
   unsigned long long r_visited_cnt_g;    // several fragments: vertices visited so far in the whole graph (resume state)
   unsigned long long t_kstart, t_kend;   // GL_TRACE: first / last instruction of the fused multi-fragment kernel (thread 0)
-  unsigned long long xt[8];      // GL_TRACE: timestamps inside the most recent xsync (block 0, thread 0)   // GL_TRACE: phase timestamps of the first 32 levels (thread 0)
+  unsigned long long xt[8];      // GL_TRACE: timestamps inside the most recent xsync (block 0, thread 0)
   uint32_t x_error, x_pad;   // 1 = a peer did not show up in time, 2 = landing slot overflow
   BfsLevelStat stat[kMaxFusedStats];
 };
@@ -699,36 +697,79 @@ GL_DEV unsigned long long global_ns() {
   return t;
 }
 
+// When a pull phase keeps pulling although its frontier has become small (the tail of the query).
+enum BfsTailRule : uint32_t {
+  kNoTail,            // never: back to push
+  kTailPerFrontier,   // while few candidates remain per frontier vertex (unvisited <= 64 n_f)
+  kTailAbsolute,      // ... or few in absolute terms (unvisited <= V / 64)
+};
+
+// The push/pull schedule of every query path (both fused kernels and the stepwise host loop).
 // push -> pull when the frontier's edges exceed 1/14 of the unvisited edges;
-// pull -> push (for good) when the frontier shrinks below V/24 (Beamer et
+// pull -> push (for good) when the frontier shrinks below V/beta (Beamer et
 // al.; the reference uses vertex ratios, bfs.h:171-180 — the schedule only
 // affects speed, never the levels).  phase: 0 = initial push, 1 = pull,
 // 2 = final push; k_bfs_fused adds kListPull = pull over the tail candidate
 // list, kept until the query ends (never an input of bfs_next_phase).
+// `tail` is a constant at every call site, so each caller compiles only its own rule.
 constexpr uint32_t kListPull = 3;
-GL_DEV uint32_t bfs_next_phase(uint32_t phase, unsigned long long n_f,
-                               unsigned long long m_f, unsigned long long m_u,
-                               uint32_t ivnum, int direction_opt, uint32_t beta,
-                               unsigned long long unvisited_nz) {
+__host__ __device__ __forceinline__ uint32_t bfs_next_phase(uint32_t phase, unsigned long long n_f, unsigned long long m_f,
+                                                            unsigned long long m_u, unsigned long long vnum,
+                                                            int direction_opt, uint32_t beta,
+                                                            unsigned long long unvisited, BfsTailRule tail) {
   if (!direction_opt) return 0;
   if (phase == 0) return m_f > m_u / 14 ? 1u : 0u;
   if (phase == 1) {
     // A pull level costs ~ the unvisited non-isolated vertices, a push level
     // ~ the frontier's edges plus two grid barriers: keep pulling while the
-    // frontier is large (Beamer) or while few candidates remain per frontier
-    // vertex (the tail of a skewed graph); go back to push for long sparse tails.
-    // n_f >= floor(ivnum / beta), without a division the compiler would hoist out of the level loop
+    // frontier is large (Beamer) or, per `tail`, while few candidates remain;
+    // go back to push for long sparse tails.
+    // n_f >= floor(vnum / beta), without a division the compiler would hoist out of the level loop
     // and keep live (k_bfs_fused has no register to spare)
-    if ((n_f + 1) * beta > ivnum) return 1u;
-    return unvisited_nz <= 64ull * n_f ? 1u : 2u;
+    if ((n_f + 1) * beta > vnum) return 1u;
+    if (tail != kNoTail && unvisited <= 64ull * n_f) return 1u;
+    if (tail == kTailAbsolute && unvisited <= vnum / 64) return 1u;
+    return 2u;
   }
   return 2u;
 }
 
+// The state a launch of a fused kernel parks when the level ring is full: the host spills levels
+// [0, max_lv-1) and relaunches from it (k_bfs_resume_prep).  A tail list does not survive the
+// relaunch: its first level sweeps the bitmap again.
+GL_DEV void bfs_park(BfsFusedCtl* ctl, unsigned long long n_f, unsigned long long m_f, unsigned long long visited_edges,
+                     unsigned long long visited_cnt, uint32_t phase) {
+  ctl->overflow = 1;
+  ctl->p_nf = n_f;
+  ctl->p_mf = m_f;
+  ctl->p_visited_edges = visited_edges;
+  ctl->p_visited_cnt = visited_cnt;
+  ctl->p_phase = phase == kListPull ? 1u : phase;
+}
+
+// Thread 0's bookkeeping at the end of level `depth` of a fused kernel: the level's statistics
+// (`frontier` vertices expanded, `mode` 1 = pull), the level count and the counters of the query;
+// c[(depth+2)%3] was last read during this level and is cleared for level depth+1.
+GL_DEV void bfs_level_end(BfsFusedCtl* ctl, uint32_t depth_base, uint32_t depth, unsigned long long frontier,
+                          uint32_t mode) {
+  const volatile ScanCtrl* VC = &ctl->c[depth % 3];
+  const uint32_t adepth = depth_base + depth;
+  if (adepth < (uint32_t) kMaxFusedStats) {
+    BfsLevelStat ls;
+    ls.t_ns = global_ns();
+    ls.scanned = VC->scanned;
+    ls.frontier = (uint32_t) (frontier > 0xFFFFFFFFull ? 0xFFFFFFFFull : frontier);
+    ls.mode = mode;
+    ctl->stat[adepth] = ls;
+  }
+  ctl->levels = adepth + 1;
+  ctl->touched += VC->touched;
+  ctl->c[(depth + 2) % 3] = ScanCtrl();
+}
+
 // first launch of a several-fragment query (k_bfs_fused_multi); k_bfs_fused seeds itself
-__global__ void k_bfs_seed_fused(uint32_t src, int has_src, uint32_t* lv0,
-                                 uint32_t* vis, const uint64_t* rp,
-                                 unsigned long long m_total, BfsFusedCtl* ctl) {
+__global__ void k_bfs_seed_fused(uint32_t src, int has_src, uint32_t* lv0, uint32_t* vis, const uint64_t* rp,
+                                 BfsFusedCtl* ctl) {
   if (blockIdx.x != 0 || threadIdx.x != 0) return;
   ctl->c[0] = ScanCtrl();
   ctl->c[1] = ScanCtrl();
@@ -736,7 +777,6 @@ __global__ void k_bfs_seed_fused(uint32_t src, int has_src, uint32_t* lv0,
   ctl->levels = 0;
   ctl->overflow = 0;
   ctl->touched = 0;
-  ctl->m_total = m_total;
   unsigned long long deg = 0;
   if (has_src) {
     lv0[src >> 5] |= 1u << (src & 31);
@@ -745,7 +785,6 @@ __global__ void k_bfs_seed_fused(uint32_t src, int has_src, uint32_t* lv0,
   }
   ctl->has_src = has_src;
   ctl->src_lid = src;
-  ctl->src_deg = deg;
   ctl->r_nf = has_src ? 1 : 0;
   ctl->r_mf = deg;
   ctl->r_visited_edges = deg;
@@ -773,19 +812,23 @@ __global__ void k_bfs_resume_prep(BfsFusedCtl* ctl) {
   ctl->r_phase = ctl->p_phase;
 }
 
+// the first of ring levels [0, nlevels) whose bitmap holds bit i; nlevels when none does
+// (coalesced: the threads of a warp share words)
+GL_DEV uint32_t bfs_first_level(const uint32_t* lv, uint32_t words, uint32_t nlevels, uint32_t i) {
+  const uint32_t w = i >> 5, m = 1u << (i & 31);
+  uint32_t l = 0;
+  while (l < nlevels && !(lv[(size_t) l * words + w] & m)) ++l;
+  return l;
+}
+
 // Spill: depth of every vertex found in ring levels [0, nlevels) goes to the
 // int32 side array (absolute depth = base + ring index).
 __global__ void k_bfs_spill(const uint32_t* lv, uint32_t words, uint32_t nlevels, uint32_t n,
                             uint32_t base, int32_t* spill) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const uint32_t w = i >> 5, m = 1u << (i & 31);
-  for (uint32_t l = 0; l < nlevels; ++l) {
-    if (lv[(size_t) l * words + w] & m) {
-      spill[i] = (int32_t) (base + l);
-      break;
-    }
-  }
+  const uint32_t l = bfs_first_level(lv, words, nlevels, i);
+  if (l < nlevels) spill[i] = (int32_t) (base + l);
 }
 
 struct BfsFusedArgs {
@@ -924,7 +967,8 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
     const unsigned long long deg = a.has_src ? a.er.rp[a.src + 1] - a.er.rp[a.src] : 0ull;
     n_f = visited_cnt = a.has_src ? 1ull : 0ull;
     m_f = visited_edges = deg;
-    phase = bfs_next_phase(0, n_f, m_f, m_total - visited_edges, a.pa.ivnum, a.direction_opt, a.beta, a.nz_total);
+    phase = bfs_next_phase(0, n_f, m_f, m_total - visited_edges, a.pa.ivnum, a.direction_opt, a.beta, a.nz_total,
+                           kTailPerFrontier);
     if (gtid == 0) {
       ctl->t_begin = global_ns();
       if (a.has_src) {
@@ -944,16 +988,7 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
   }
   for (uint32_t depth = 0; n_f != 0; ++depth) {
     if (depth + 1 >= a.max_lv) {
-      // ring full: park the state; the host spills levels [0, max_lv-1) and relaunches (the tail
-      // list does not survive the relaunch: its first level sweeps the bitmap again)
-      if (gtid == 0) {
-        ctl->overflow = 1;
-        ctl->p_nf = n_f;
-        ctl->p_mf = m_f;
-        ctl->p_visited_edges = visited_edges;
-        ctl->p_visited_cnt = visited_cnt;
-        ctl->p_phase = phase == kListPull ? 1u : phase;
-      }
+      if (gtid == 0) bfs_park(ctl, n_f, m_f, visited_edges, visited_cnt, phase);
       break;
     }
     ScanCtrl* C = &ctl->c[depth % 3];
@@ -991,21 +1026,7 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
     const unsigned long long next_edges = VC->next_edges;
     const bool listed = (phase == kListPull || (phase == 1 && a.pa.list_cap && a.nz_total <= visited_cnt + a.list_gap)) &&
                         VC->aux_ticket <= a.pa.list_cap;
-    if (gtid == 0) {
-      const uint32_t adepth = a.depth_base + depth;
-      if (adepth < (uint32_t) kMaxFusedStats) {
-        BfsLevelStat ls;
-        ls.t_ns = global_ns();
-        ls.scanned = VC->scanned;
-        ls.frontier = (uint32_t) (n_f > 0xFFFFFFFFull ? 0xFFFFFFFFull : n_f);
-        ls.mode = (phase == 1 || phase == kListPull) ? 1u : 0u;
-        ctl->stat[adepth] = ls;
-      }
-      ctl->levels = adepth + 1;
-      ctl->touched += VC->touched;
-      // c[(depth+2)%3] was last read during this level
-      ctl->c[(depth + 2) % 3] = ScanCtrl();
-    }
+    if (gtid == 0) bfs_level_end(ctl, a.depth_base, depth, n_f, (phase == 1 || phase == kListPull) ? 1u : 0u);
     n_f = next_count;
     m_f = next_edges;
     visited_edges += next_edges;
@@ -1016,7 +1037,7 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
                    : bfs_next_phase(phase, n_f, m_f,
                                     m_total > visited_edges ? m_total - visited_edges : 0,
                                     a.pa.ivnum, a.direction_opt, a.beta,
-                                    a.nz_total > visited_cnt ? a.nz_total - visited_cnt : 0);
+                                    a.nz_total > visited_cnt ? a.nz_total - visited_cnt : 0, kTailPerFrontier);
   }
 }
 
@@ -1338,30 +1359,19 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused_multi(BfsM
   for (uint32_t depth = 0; n_f != 0; ++depth) {
     if (depth + 1 >= a.max_lv) {
       if (gtid == 0) {
-        ctl->overflow = 1;
-        ctl->p_nf = n_f;
-        ctl->p_mf = m_f;
-        ctl->p_visited_edges = visited_edges;
-        ctl->p_visited_cnt = 0;
+        bfs_park(ctl, n_f, m_f, visited_edges, 0, phase);
         ctl->r_visited_cnt_g = visited_cnt;
-        ctl->p_phase = phase;
       }
       break;
     }
-    // direction on WHOLE-GRAPH statistics (identical on every GPU)
+    // direction on WHOLE-GRAPH statistics (identical on every GPU).  Only the global-frontier scheme,
+    // whose pull levels exchange no per-vertex messages, keeps pulling in the tail (a push level after
+    // the pulls re-reports every outer neighbour of its frontier), also while fewer than V/64 candidates
+    // remain: such a pull costs less than a push level's pack + message round + apply.
     const unsigned long long m_u = A.g_m_total > visited_edges ? A.g_m_total - visited_edges : 0;
-    uint32_t nphase = 0;
-    if (!a.direction_opt) nphase = 0;
-    else if (phase == 0) nphase = (m_f > m_u / 14) ? 1u : 0u;
-    else if (phase == 1) {
-      // as on one GPU (bfs_next_phase): keep pulling while the frontier is large, or -- global-frontier
-      // scheme, whose pull levels exchange no per-vertex messages -- while few candidates remain per
-      // frontier vertex; a push level after the pulls re-reports every outer neighbour of its frontier
-      const unsigned long long unvis = A.g_nz_total > visited_cnt ? A.g_nz_total - visited_cnt : 0;
-      // ... or in absolute terms (the tail of the query: a pull over < V/64 candidates costs less than a
-      // push level's pack + message round + apply)
-      nphase = (n_f >= A.g_vnum / a.beta) ? 1u : ((kGF && (unvis <= 64ull * n_f || unvis <= A.g_vnum / 64)) ? 1u : 2u);
-    } else nphase = 2;
+    const unsigned long long unvis = A.g_nz_total > visited_cnt ? A.g_nz_total - visited_cnt : 0;
+    const uint32_t nphase = bfs_next_phase(phase, n_f, m_f, m_u, A.g_vnum, a.direction_opt, a.beta, unvis,
+                                           kGF ? kTailAbsolute : kNoTail);
     ScanCtrl* C = &ctl->c[depth % 3];
     uint32_t* cur = a.lv + (size_t) depth * a.words;
     uint32_t* nxt = a.lv + (size_t) (depth + 1) * a.words;
@@ -1535,23 +1545,11 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused_multi(BfsM
         ctl->xw[tl][0] = ctl->xt[3] - ctl->xt[2];
         ctl->xw[tl][1] = ctl->xt[1] - ctl->xt[0];
       }
-      const volatile ScanCtrl* VC = C;
-      const uint32_t adepth = a.depth_base + depth;
-      if (adepth < (uint32_t) kMaxFusedStats) {
-        BfsLevelStat ls;
-        ls.t_ns = global_ns();
-        ls.scanned = VC->scanned;
-        // THIS fragment's share of the level's frontier (n_f is the whole graph's): what it found in the
-        // previous level (vertices that arrived as messages in a push level are not counted)
-        const unsigned long long l_nf = ctl->l_nf;
-        ls.frontier = (uint32_t) (l_nf > 0xFFFFFFFFull ? 0xFFFFFFFFull : l_nf);
-        ls.mode = phase == 1 ? 1u : 0u;
-        ctl->stat[adepth] = ls;
-      }
-      ctl->l_nf = VC->next_count;
-      ctl->levels = adepth + 1;
-      ctl->touched += VC->touched;
-      ctl->c[(depth + 2) % 3] = ScanCtrl();
+      // the statistics record THIS fragment's share of the level's frontier (n_f is the whole graph's):
+      // what it found in the previous level (vertices that arrived as messages in a push level are not
+      // counted)
+      bfs_level_end(ctl, a.depth_base, depth, ctl->l_nf, phase == 1 ? 1u : 0u);
+      ctl->l_nf = ((const volatile ScanCtrl*) C)->next_count;
       ctl->x_msg_rounds = msg_round - x.msg_round0;
       ctl->x_mirror_syncs = mseq - x.mirror_seq0;
     }
@@ -1577,7 +1575,7 @@ struct BfsApply {
   }
 };
 
-// depth[v] = first level whose bitmap holds v (coalesced: a warp shares words)
+// depth[v] = first level whose bitmap holds v
 // (perm != null: the bitmaps are indexed by the hub-first rank of the vertex)
 // (spill != null: levels older than `base` were moved to the side array)
 __global__ void k_depth_from_levels(const uint32_t* lv, uint32_t words,
@@ -1585,20 +1583,13 @@ __global__ void k_depth_from_levels(const uint32_t* lv, uint32_t words,
                                     uint32_t base, const int32_t* spill, int64_t* out) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  int64_t d = INT64_MAX;
   const uint32_t pi = perm ? perm[i] : i;
-  const uint32_t w = pi >> 5, m = 1u << (pi & 31);
   if (spill && spill[pi] >= 0) {
     out[i] = spill[pi];
     return;
   }
-  for (uint32_t l = 0; l < nlevels; ++l) {
-    if (lv[(size_t) l * words + w] & m) {
-      d = (int64_t) base + l;
-      break;
-    }
-  }
-  out[i] = d;
+  const uint32_t l = bfs_first_level(lv, words, nlevels, pi);
+  out[i] = l < nlevels ? (int64_t) base + l : INT64_MAX;
 }
 
 // depth as ONE byte per vertex (0xFF = unreached): 8x fewer bytes across PCIe
@@ -1607,16 +1598,8 @@ __global__ void k_depth_u8_from_levels(const uint32_t* lv, uint32_t words, uint3
                                        const uint32_t* perm, uint8_t* out) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const uint32_t pi = perm ? perm[i] : i;
-  const uint32_t w = pi >> 5, m = 1u << (pi & 31);
-  uint32_t d = 0xFFu;
-  for (uint32_t l = 0; l < nlevels; ++l) {
-    if (lv[(size_t) l * words + w] & m) {
-      d = l;
-      break;
-    }
-  }
-  out[i] = (uint8_t) d;
+  const uint32_t l = bfs_first_level(lv, words, nlevels, perm ? perm[i] : i);
+  out[i] = (uint8_t) (l < nlevels ? l : 0xFFu);
 }
 
 struct BfsApp : gl_app {
@@ -1671,9 +1654,8 @@ struct BfsApp : gl_app {
   size_t ResultElemBytes() const override { return sizeof(int64_t); }
 
   uint32_t* level_bm(uint32_t d) { return lv + (size_t) d * words; }
-  // pull scans whole rows: with several fragments the frontier bits of the
-  // outer copies are refreshed from their owners first (mirror sync)
-  const uint64_t* row_end() const { return p_rp + 1; }
+  // pull -> push when the frontier shrinks below V / beta (bfs_next_phase), on every query path
+  uint32_t beta() const { return cfg.reserved[2] > 0 ? (uint32_t) cfg.reserved[2] : 24u; }
 
   // The pull step walks the INCOMING adjacency (bfs.h:225-238): `ie` when the
   // fragment is directed, the (aliased) `oe` when it is not.  A directed
@@ -1696,6 +1678,31 @@ struct BfsApp : gl_app {
     return GL_OK;
   }
 
+  // Several fragments, replicated global frontier: gid-space copies of the pull adjacency (gcol) and of
+  // the hub-neighbour table (hub_nbr_g); `ovgid` = the gids of the outer copies.  sorted: the rows are
+  // re-sorted by rank key and hub_nbr_g is read off their first column (hub-first order); otherwise
+  // hub_nbr_g maps hub_nbr.
+  int BuildGidPull(const uint32_t* ovgid, bool sorted) {
+    const uint64_t m = fv.directed ? frag->ie.entries : frag->oe.entries;
+    const uint32_t gid0 = fv.fid << fv.fid_offset;
+    GL_CUDA(gcol.alloc(m + 16));
+    GL_CUDA(hub_nbr_g.alloc((size_t) fv.ivnum + kSuperV));
+    GL_CUDA(cudaMemsetAsync(hub_nbr_g, 0xFF, sizeof(uint32_t) * ((size_t) fv.ivnum + kSuperV), eng.stream));
+    if (m) GL_LAUNCH(k_bfs_gcol, eng.sm_count * 8, 256, eng.stream, p_col, m, fv.ivnum, gid0, ovgid, gcol);
+    if (sorted && m) {
+      GL_LAUNCH(k_bfs_gid_key, eng.sm_count * 8, 256, eng.stream, gcol, m, fv.fid_offset, fv.id_mask, 1);
+      GL_TRY(sort_csr_rows(eng.stream, p_rp, fv.ivnum, m, &gcol));
+      GL_LAUNCH(k_bfs_gid_key, eng.sm_count * 8, 256, eng.stream, gcol, m, fv.fid_offset, fv.id_mask, 0);
+    }
+    if (!fv.ivnum) return GL_OK;
+    // the first entry of a sorted row is its highest-ranked neighbour: the stage-1 probe of the pull
+    if (sorted) GL_LAUNCH(k_bfs_first_col, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, gcol, fv.ivnum, hub_nbr_g);
+    else GL_LAUNCH(k_bfs_gid_table, (fv.ivnum + 255) / 256, 256, eng.stream, hub_nbr, fv.ivnum, fv.ivnum, gid0, ovgid, hub_nbr_g);
+    return GL_OK;
+  }
+
+  // Decide the vertex order first (one fragment: on local facts; several: on the collective totals),
+  // then build the adjacency, its tables and the statistics once, on that order.
   int Setup() override {
     tvnum = fv.ivnum + fv.ovnum;
     words = (bm_words(tvnum) + 4) & ~(size_t) 3;
@@ -1718,52 +1725,14 @@ struct BfsApp : gl_app {
     g_nz = frag->nonzero_deg;
     // the source is fixed per app (AppConfig): resolve it once
     has_src_ = gl_frag_oid2lid(frag, cfg.source_oid, &src_) == GL_OK ? 1 : 0;
-    // hub-first shadow graph (one fragment, undirected, large enough to matter)
-    if (fv.fnum == 1 && can_pull() && !fv.directed && ((fv.ivnum >= (1u << 16) && cfg.reserved[1] == 0) || cfg.reserved[1] == 2))
-      GL_TRY(BuildHubFirst());
-    if (fv.ivnum && cfg.direction_opt) {
-      GL_CUDA(deg8.alloc(fv.ivnum));
-      GL_LAUNCH(k_bfs_deg8, (fv.ivnum + 255) / 256, 256, eng.stream, g_rp, fv.ivnum, deg8);
-    }
-    p_rp = g_rp;
-    p_col = g_col;
-    if (fv.directed && can_pull()) {
-      p_rp = fv.ie_rp;
-      p_col = fv.ie_col;
-      GL_CUDA(nz_in.alloc(words));
-      GL_CUDA(cudaMemsetAsync(nz_in, 0, sizeof(uint32_t) * words, eng.stream));
-      if (fv.ivnum) GL_LAUNCH(k_bfs_nz, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, fv.ivnum, nz_in);
-      g_nz = nz_in;   // pull candidates / "still reachable" statistics: in-degree > 0
-    }
-    if (fv.ivnum && can_pull()) {
-      // hub-first order: the first entry of a sorted row is its highest-degree neighbour, and the pull
-      // relies on hub_nbr[v] being that entry (stage 2 starts after it)
-      if (perm) GL_LAUNCH(k_bfs_first_col, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, p_col, fv.ivnum, hub_nbr);
-      else GL_LAUNCH(k_bfs_hub_nbr, eng.sm_count * 8, 256, eng.stream, p_rp, row_end(), p_col, fv.ivnum, hub_nbr);
-    }
-    {
-      DevBuf<unsigned long long> d_cnt;
-      GL_CUDA(d_cnt.alloc(2));
-      GL_CUDA(cudaMemsetAsync(d_cnt, 0, 16, eng.stream));
-      GL_LAUNCH(k_bfs_popc, eng.sm_count * 4, 256, eng.stream, g_nz, (uint32_t) bm_words(fv.ivnum), d_cnt);
-      GL_CUDA(cudaMemcpyAsync(&nz_total, d_cnt, 8, cudaMemcpyDeviceToHost, eng.stream));
-      if (perm) {
-        // descending degree: the rows of two or more entries are a prefix of the lids
-        unsigned long long m2 = 0;
-        GL_LAUNCH(k_bfs_count_rows, eng.sm_count * 4, 256, eng.stream, p_rp, fv.ivnum, (uint64_t) 2, d_cnt + 1);
-        GL_CUDA(cudaMemcpyAsync(&m2, d_cnt + 1, 8, cudaMemcpyDeviceToHost, eng.stream));
-        GL_CUDA(cudaStreamSynchronize(eng.stream));
-        multi_v = (uint32_t) m2;
-        GL_CUDA(tail_list.alloc(kTailList));
-      }
-      GL_CUDA(cudaStreamSynchronize(eng.stream));
-    }
-    GL_CUDA(cudaStreamSynchronize(eng.stream));
     used_lv = 0;
     // message = bare lid (bfs.h:50-51: sizeof(vid_t) per outer vertex)
     GL_TRY(mm.Init(comm, fv, sizeof(ItemU32)));
     g_m_total = frag->oe.entries;
     g_vnum = fv.ivnum;
+    // hub-first shadow graph (one fragment, undirected, large enough to matter)
+    bool hub_first = fv.fnum == 1 && can_pull() && !fv.directed &&
+                     ((fv.ivnum >= (1u << 16) && cfg.reserved[1] == 0) || cfg.reserved[1] == 2);
     if (fv.fnum > 1) {
       GL_TRY(mm.BuildMirrorPlan(eng.stream, fv));
       long long a = (long long) frag->oe.entries, b = (long long) fv.ivnum;
@@ -1771,11 +1740,6 @@ struct BfsApp : gl_app {
       GL_TRY(mm.PeerAllReduce(eng.stream, &a, &b, &c, 0));
       g_m_total = (uint64_t) a;
       g_vnum = (uint64_t) b;
-      {
-        long long z = (long long) nz_total, z2 = 0;
-        GL_TRY(mm.PeerAllReduce(eng.stream, &z, &z2, &c, 0));
-        g_nz_total = (uint64_t) z;
-      }
       // every GPU must spill its level ring at the same depth
       long long lo = (long long) max_lv, dummy = 0;
       GL_TRY(mm.PeerAllReduce(eng.stream, &lo, &dummy, &c, 1));
@@ -1798,79 +1762,102 @@ struct BfsApp : gl_app {
       // one also on small graphs (tests).
       hub_multi = global_front && fused() && !fv.directed &&
                   ((cfg.reserved[1] == 0 && g_vnum >= (1u << 16)) || cfg.reserved[1] == 2 || cfg.reserved[1] == 3);
-      if (hub_multi) {
-        const uint64_t m = frag->oe.entries;
-        GL_TRY(BuildHubFirst());
-        p_rp = g_rp;
-        p_col = g_col;
-        if (deg8 && fv.ivnum) GL_LAUNCH(k_bfs_deg8, (fv.ivnum + 255) / 256, 256, eng.stream, g_rp, fv.ivnum, deg8);
-        // owners' new lids reach the outer copies through one dense mirror sync
-        DevBuf<uint32_t> newlid;
-        GL_CUDA(newlid.alloc(std::max<size_t>(tvnum, 1)));
-        GL_CUDA(cudaMemsetAsync(newlid, 0, sizeof(uint32_t) * std::max<size_t>(tvnum, 1), eng.stream));
-        if (fv.ivnum) GL_CUDA(cudaMemcpyAsync(newlid, perm, sizeof(uint32_t) * fv.ivnum, cudaMemcpyDeviceToDevice, eng.stream));
-        GL_TRY(mm.SyncValuesToGhosts(eng.stream, newlid, 4));
-        GL_CUDA(ovgid_p.alloc(std::max<uint32_t>(fv.ovnum, 1)));
-        if (fv.ovnum)
-          GL_LAUNCH(k_bfs_ovgid_new, (fv.ovnum + 255) / 256, 256, eng.stream, fv.ovgid, newlid + fv.ivnum, fv.ovnum, fv.id_mask, ovgid_p);
-        const uint32_t gid0 = fv.fid << fv.fid_offset;
-        GL_CUDA(gcol.alloc(m + 16));
-        GL_CUDA(hub_nbr_g.alloc((size_t) fv.ivnum + kSuperV));
-        GL_CUDA(cudaMemsetAsync(hub_nbr_g, 0xFF, sizeof(uint32_t) * ((size_t) fv.ivnum + kSuperV), eng.stream));
-        if (m) {
-          GL_LAUNCH(k_bfs_gcol, eng.sm_count * 8, 256, eng.stream, p_col, m, fv.ivnum, gid0, ovgid_p, gcol);
-          GL_LAUNCH(k_bfs_gid_key, eng.sm_count * 8, 256, eng.stream, gcol, m, fv.fid_offset, fv.id_mask, 1);
-          GL_TRY(sort_csr_rows(eng.stream, p_rp, fv.ivnum, m, &gcol));
-          GL_LAUNCH(k_bfs_gid_key, eng.sm_count * 8, 256, eng.stream, gcol, m, fv.fid_offset, fv.id_mask, 0);
-        }
-        // the first entry of a sorted row is its highest-ranked neighbour: the stage-1 probe of the pull
-        if (fv.ivnum) GL_LAUNCH(k_bfs_first_col, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, gcol, fv.ivnum, hub_nbr_g);
-        if (cfg.reserved[1] != 3) {   // ([1] = 3: hub-first order without the delegated hubs, A/B)
-          const uint32_t K = fv.fnum * kDlgPerFrag;
-          DevBuf<uint32_t> cnt;
-          GL_CUDA(cnt.alloc(K));
-          GL_CUDA(cudaMemsetAsync(cnt, 0, sizeof(uint32_t) * K, eng.stream));
-          if (fv.ivnum)
-            GL_LAUNCH(k_bfs_dlg_scan, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, gcol, fv.ivnum, fv.fid_offset, fv.id_mask, cnt,
-                      nullptr, nullptr, 0);
-          std::vector<uint32_t> h_cnt(K);
-          GL_CUDA(cudaMemcpyAsync(h_cnt.data(), cnt, sizeof(uint32_t) * K, cudaMemcpyDeviceToHost, eng.stream));
-          GL_CUDA(cudaStreamSynchronize(eng.stream));
-          std::vector<uint64_t> h_off(K + 1, 0);
-          for (uint32_t h = 0; h < K; ++h) h_off[h + 1] = h_off[h] + h_cnt[h];
-          GL_CUDA(dlg_off.alloc(K + 1));
-          GL_CUDA(cudaMemcpyAsync(dlg_off, h_off.data(), sizeof(uint64_t) * (K + 1), cudaMemcpyHostToDevice, eng.stream));
-          GL_CUDA(dlg_list.alloc(h_off[K] + 16));
-          GL_CUDA(cudaMemsetAsync(cnt, 0, sizeof(uint32_t) * K, eng.stream));
-          if (fv.ivnum)
-            GL_LAUNCH(k_bfs_dlg_scan, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, gcol, fv.ivnum, fv.fid_offset, fv.id_mask, cnt,
-                      dlg_off, dlg_list, 1);
-          GL_TRY(sort_csr_rows(eng.stream, dlg_off, K, h_off[K], &dlg_list));   // ascending lid: neighbouring bits, neighbouring words
-          GL_CUDA(cudaStreamSynchronize(eng.stream));
-        }
-        GL_CUDA(cudaStreamSynchronize(eng.stream));
-      } else if (can_pull() && fv.ivnum + fv.ovnum) {
-        // the hub-neighbour prefilter should pick the true highest-degree neighbour, also when it is an
-        // outer copy: owners' degrees reach the ghosts through one dense mirror sync (collective)
-        DevBuf<uint32_t> deg32;
-        GL_CUDA(deg32.alloc(tvnum));
-        GL_LAUNCH(k_bfs_deg32, (tvnum + 255) / 256, 256, eng.stream, fv.oe_rp, fv.ivnum, tvnum, deg32);
-        GL_TRY(mm.SyncValuesToGhosts(eng.stream, deg32, 4));
-        if (fv.ivnum) GL_LAUNCH(k_bfs_hub_nbr, eng.sm_count * 8, 256, eng.stream, p_rp, row_end(), p_col, fv.ivnum, hub_nbr, deg32);
-        GL_CUDA(cudaStreamSynchronize(eng.stream));
-      } else if (can_pull()) {
-        GL_TRY(mm.SyncValuesToGhosts(eng.stream, nullptr, 4));   // keep the collective sequence identical on every rank
+      hub_first = hub_multi;
+    }
+    if (hub_first) GL_TRY(BuildHubFirst());
+    p_rp = g_rp;
+    p_col = g_col;
+    if (fv.directed && can_pull()) {
+      p_rp = fv.ie_rp;
+      p_col = fv.ie_col;
+      GL_CUDA(nz_in.alloc(words));
+      GL_CUDA(cudaMemsetAsync(nz_in, 0, sizeof(uint32_t) * words, eng.stream));
+      if (fv.ivnum) GL_LAUNCH(k_bfs_nz, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, fv.ivnum, nz_in);
+      g_nz = nz_in;   // pull candidates / "still reachable" statistics: in-degree > 0
+    }
+    if (fv.ivnum && cfg.direction_opt) {
+      GL_CUDA(deg8.alloc(fv.ivnum));
+      GL_LAUNCH(k_bfs_deg8, (fv.ivnum + 255) / 256, 256, eng.stream, g_rp, fv.ivnum, deg8);
+    }
+    if (fv.fnum == 1 && fv.ivnum && can_pull()) {
+      // hub-first order: the first entry of a sorted row is its highest-degree neighbour, and the pull
+      // relies on hub_nbr[v] being that entry (stage 2 starts after it)
+      if (perm) GL_LAUNCH(k_bfs_first_col, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, p_col, fv.ivnum, hub_nbr);
+      else GL_LAUNCH(k_bfs_hub_nbr, eng.sm_count * 8, 256, eng.stream, p_rp, p_col, fv.ivnum, hub_nbr);
+    }
+    {
+      DevBuf<unsigned long long> d_cnt;
+      GL_CUDA(d_cnt.alloc(2));
+      GL_CUDA(cudaMemsetAsync(d_cnt, 0, 16, eng.stream));
+      GL_LAUNCH(k_bfs_popc, eng.sm_count * 4, 256, eng.stream, g_nz, (uint32_t) bm_words(fv.ivnum), d_cnt);
+      GL_CUDA(cudaMemcpyAsync(&nz_total, d_cnt, 8, cudaMemcpyDeviceToHost, eng.stream));
+      unsigned long long m2 = 0;
+      if (fv.fnum == 1 && perm) {
+        // descending degree: the rows of two or more entries are a prefix of the lids
+        GL_LAUNCH(k_bfs_count_rows, eng.sm_count * 4, 256, eng.stream, p_rp, fv.ivnum, (uint64_t) 2, d_cnt + 1);
+        GL_CUDA(cudaMemcpyAsync(&m2, d_cnt + 1, 8, cudaMemcpyDeviceToHost, eng.stream));
+        GL_CUDA(tail_list.alloc(kTailList));
       }
-      if (global_front && !hub_multi) {
-        const uint64_t m = (fv.directed ? frag->ie.entries : frag->oe.entries);
-        const uint32_t gid0 = fv.fid << fv.fid_offset;
-        GL_CUDA(gcol.alloc(m + 16));
-        GL_CUDA(hub_nbr_g.alloc((size_t) fv.ivnum + kSuperV));
-        GL_CUDA(cudaMemsetAsync(hub_nbr_g, 0xFF, sizeof(uint32_t) * ((size_t) fv.ivnum + kSuperV), eng.stream));
-        if (m) GL_LAUNCH(k_bfs_gcol, eng.sm_count * 8, 256, eng.stream, p_col, m, fv.ivnum, gid0, fv.ovgid, gcol);
-        if (fv.ivnum) GL_LAUNCH(k_bfs_gid_table, (fv.ivnum + 255) / 256, 256, eng.stream, hub_nbr, fv.ivnum, fv.ivnum, gid0, fv.ovgid, hub_nbr_g);
+      GL_CUDA(cudaStreamSynchronize(eng.stream));
+      multi_v = (uint32_t) m2;
+    }
+    if (fv.fnum == 1) return GL_OK;
+    {
+      long long z = (long long) nz_total, z2 = 0;
+      double c = 0;
+      GL_TRY(mm.PeerAllReduce(eng.stream, &z, &z2, &c, 0));
+      g_nz_total = (uint64_t) z;
+    }
+    if (hub_multi) {
+      // owners' new lids reach the outer copies through one dense mirror sync
+      DevBuf<uint32_t> newlid;
+      GL_CUDA(newlid.alloc(std::max<size_t>(tvnum, 1)));
+      GL_CUDA(cudaMemsetAsync(newlid, 0, sizeof(uint32_t) * std::max<size_t>(tvnum, 1), eng.stream));
+      if (fv.ivnum) GL_CUDA(cudaMemcpyAsync(newlid, perm, sizeof(uint32_t) * fv.ivnum, cudaMemcpyDeviceToDevice, eng.stream));
+      GL_TRY(mm.SyncValuesToGhosts(eng.stream, newlid, 4));
+      GL_CUDA(ovgid_p.alloc(std::max<uint32_t>(fv.ovnum, 1)));
+      if (fv.ovnum)
+        GL_LAUNCH(k_bfs_ovgid_new, (fv.ovnum + 255) / 256, 256, eng.stream, fv.ovgid, newlid + fv.ivnum, fv.ovnum, fv.id_mask, ovgid_p);
+      GL_TRY(BuildGidPull(ovgid_p, true));
+      if (cfg.reserved[1] != 3) {   // ([1] = 3: hub-first order without the delegated hubs, A/B)
+        const uint32_t K = fv.fnum * kDlgPerFrag;
+        DevBuf<uint32_t> cnt;
+        GL_CUDA(cnt.alloc(K));
+        GL_CUDA(cudaMemsetAsync(cnt, 0, sizeof(uint32_t) * K, eng.stream));
+        if (fv.ivnum)
+          GL_LAUNCH(k_bfs_dlg_scan, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, gcol, fv.ivnum, fv.fid_offset, fv.id_mask, cnt,
+                    nullptr, nullptr, 0);
+        std::vector<uint32_t> h_cnt(K);
+        GL_CUDA(cudaMemcpyAsync(h_cnt.data(), cnt, sizeof(uint32_t) * K, cudaMemcpyDeviceToHost, eng.stream));
+        GL_CUDA(cudaStreamSynchronize(eng.stream));
+        std::vector<uint64_t> h_off(K + 1, 0);
+        for (uint32_t h = 0; h < K; ++h) h_off[h + 1] = h_off[h] + h_cnt[h];
+        GL_CUDA(dlg_off.alloc(K + 1));
+        GL_CUDA(cudaMemcpyAsync(dlg_off, h_off.data(), sizeof(uint64_t) * (K + 1), cudaMemcpyHostToDevice, eng.stream));
+        GL_CUDA(dlg_list.alloc(h_off[K] + 16));
+        GL_CUDA(cudaMemsetAsync(cnt, 0, sizeof(uint32_t) * K, eng.stream));
+        if (fv.ivnum)
+          GL_LAUNCH(k_bfs_dlg_scan, (fv.ivnum + 255) / 256, 256, eng.stream, p_rp, gcol, fv.ivnum, fv.fid_offset, fv.id_mask, cnt,
+                    dlg_off, dlg_list, 1);
+        GL_TRY(sort_csr_rows(eng.stream, dlg_off, K, h_off[K], &dlg_list));   // ascending lid: neighbouring bits, neighbouring words
         GL_CUDA(cudaStreamSynchronize(eng.stream));
       }
+      GL_CUDA(cudaStreamSynchronize(eng.stream));
+    } else if (can_pull() && tvnum) {
+      // the hub-neighbour prefilter should pick the true highest-degree neighbour, also when it is an
+      // outer copy: owners' degrees reach the ghosts through one dense mirror sync (collective)
+      DevBuf<uint32_t> deg32;
+      GL_CUDA(deg32.alloc(tvnum));
+      GL_LAUNCH(k_bfs_deg32, (tvnum + 255) / 256, 256, eng.stream, fv.oe_rp, fv.ivnum, tvnum, deg32);
+      GL_TRY(mm.SyncValuesToGhosts(eng.stream, deg32, 4));
+      if (fv.ivnum) GL_LAUNCH(k_bfs_hub_nbr, eng.sm_count * 8, 256, eng.stream, p_rp, p_col, fv.ivnum, hub_nbr, deg32);
+      GL_CUDA(cudaStreamSynchronize(eng.stream));
+    } else if (can_pull()) {
+      GL_TRY(mm.SyncValuesToGhosts(eng.stream, nullptr, 4));   // keep the collective sequence identical on every rank
+    }
+    if (global_front && !hub_multi) {
+      GL_TRY(BuildGidPull(fv.ovgid, false));
+      GL_CUDA(cudaStreamSynchronize(eng.stream));
     }
     return GL_OK;
   }
@@ -1931,7 +1918,7 @@ struct BfsApp : gl_app {
   }
 
   PullArgs pull_args() const {
-    return PullArgs{p_rp, row_end(), p_col, hub_nbr, fv.ivnum, g_nz, nullptr, 0, 0, 0};
+    return PullArgs{p_rp, p_col, hub_nbr, fv.ivnum, g_nz, nullptr, 0, 0, 0};
   }
 
   bool fused() const {
@@ -1946,7 +1933,7 @@ struct BfsApp : gl_app {
     int has_src = has_src_;
     src = src_;   // already translated to the hub-first rank in Setup
     const bool multi = fv.fnum > 1;
-    if (multi) GL_LAUNCH(k_bfs_seed_fused, 1, 32, s, src, has_src, level_bm(0), vis, g_rp, (unsigned long long) g_m_total, d_ctl);
+    if (multi) GL_LAUNCH(k_bfs_seed_fused, 1, 32, s, src, has_src, level_bm(0), vis, g_rp, d_ctl);
     BfsFusedArgs a;
     a.pa = pull_args();
     a.er = EdgeRange{g_rp, g_col, nullptr};
@@ -1955,7 +1942,7 @@ struct BfsApp : gl_app {
     a.max_lv = max_lv;
     a.vis = vis;
     a.direction_opt = can_pull() ? 1 : 0;
-    a.beta = cfg.reserved[2] > 0 ? (uint32_t) cfg.reserved[2] : 24u;
+    a.beta = beta();
     a.nz_total = nz_total;
     a.m_total = g_m_total;
     a.ctl = d_ctl;
@@ -2159,16 +2146,12 @@ struct BfsApp : gl_app {
     // Direction choice on WHOLE-GRAPH statistics (identical on every fragment,
     // because the pull step is collective: it starts with a mirror sync).
     // n_f / m_f / visited_edges are global sums carried by the round vote.
+    // (the tail rule needs the unvisited count, which only one fragment keeps)
     const uint32_t prev_phase = phase;
     const uint64_t m_u = g_m_total > visited_edges ? g_m_total - visited_edges : 0;
-    if (!can_pull()) {
-      phase = 0;
-    } else if (phase == 0) {
-      phase = (n_f > 0 && m_f > m_u / 14) ? 1 : 0;
-    } else if (phase == 1) {
-      const uint64_t unvis = nz_total > visited_cnt ? nz_total - visited_cnt : 0;
-      phase = (n_f >= g_vnum / 24) ? 1 : ((fv.fnum == 1 && unvis <= 64 * n_f) ? 1 : 2);
-    }
+    const uint64_t unvis = nz_total > visited_cnt ? nz_total - visited_cnt : 0;
+    phase = bfs_next_phase(phase, n_f, m_f, m_u, g_vnum, can_pull() ? 1 : 0, beta(), unvis,
+                           multi ? kNoTail : kTailPerFrontier);
     const bool use_pull = phase == 1;
     EdgeRange er{g_rp, g_col, nullptr};
     if (!use_pull) {
