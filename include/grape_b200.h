@@ -403,8 +403,38 @@ typedef enum {
   GL_APP_KCORE = 8,    /* kcore/kcore.h  result: int64 entries whose other
                           endpoint survives the k-core peel (k = max_round);
                           v is in the k-core iff value >= k                   */
-  GL_APP_KCLIQUE = 9   /* kclique/kclique.h (--kclique_k = max_round), see below */
+  GL_APP_KCLIQUE = 9,  /* kclique/kclique.h (--kclique_k = max_round), see below */
+  GL_APP_BC = 10       /* bc/staged_bc_bfs.h + bc/staged_bc.h (--bc_source =
+                          source_oid)  result: gl_bc_value, see below          */
 } gl_app_kind;
+
+/* GL_APP_BC: single-source betweenness centrality, one gl_bc_value per inner vertex in lid order: the
+ * reference's Output() line `oid c sigma depth` (gl_app_result_oids gives the oid).  A directed fragment
+ * is refused at gl_app_create with GL_ERR_ARG; edge data is ignored.
+ *   depth: BFS level from the source; INT64_MAX for an unreached vertex (sigma = c = 0 there, and
+ *          everywhere when source_oid is not in the graph).
+ *   path_num (sigma): sigma(source) = 1; a depth-1 vertex has sigma = 1 however many parallel edges join
+ *          it to the source; a vertex at depth d >= 2 has the sum of sigma(u) over the CSR entries (v, u)
+ *          of its row with depth(u) = d - 1 (one term per copy of a parallel edge).  f64.
+ *   centrality (c): an f32 value, widened exactly.  For d = L (the deepest level) down to 0, every vertex
+ *          v at depth d takes cacc = f32(sum of double(t[u]) over the entries (v, u) of its row with
+ *          depth(u) = d + 1); for d > 0 c = f32(double(cacc) * sigma(v)) and
+ *          t[v] = f32((1.0 / sigma(v)) * (1.0 + double(c))); the source keeps c = cacc.
+ * Every sum is a gather over the vertex's own row in a fixed order (a short row sequentially, a long
+ * one in fixed 1024-entry chunks with fixed lane strides and shuffle tree, the chunk sums in order):
+ * the same graph gives bit-identical output on every run.  depth and sigma equal the reference's
+ * bit for bit while every sigma is below 2^53; c differs from it only by f32 summation error (the
+ * reference keeps a running f32 sum over atomics in thread order; this app rounds one f64 sum).
+ * Stats, one fragment: supersteps = forward levels + backward levels (2 (L + 1)); step i <= L is
+ * forward level i (step_frontier = level size, step_mode 0 push / 1 pull discovery), step L + 1 + j
+ * is backward level L - j (step_frontier = level size, step_mode 2); frontier_vertices = reached
+ * vertices.  Several fragments: one worker round per forward and per backward level, step_frontier
+ * is this fragment's share of the level. */
+typedef struct {
+  double centrality;
+  double path_num;
+  int64_t depth;
+} gl_bc_value;
 
 /* GL_APP_KCLIQUE: k = max_round, 3 <= k <= GL_KCLIQUE_MAX_K; a smaller or larger k and a directed
  * fragment are refused at gl_app_create with GL_ERR_ARG.  The result is ONE int64 (gl_app_result takes
@@ -430,7 +460,7 @@ typedef enum {
 
 typedef struct {
   int lb;                /* gl_lb (AppConfig::lb, cuda/app_config.h:22-27)     */
-  int64_t source_oid;    /* --bfs_source / --sssp_source                        */
+  int64_t source_oid;    /* --bfs_source / --sssp_source / --bc_source          */
   double pr_delta;       /* --pr_d                                              */
   int max_round;         /* --pr_mr / --cdlp_mr; GL_APP_KCORE: k (--kcore_k)   */
   int sssp_f64;          /* 1: fp64 distances on device (real-weight 1e-6 run)  */

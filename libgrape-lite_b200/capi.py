@@ -10,9 +10,11 @@ LIB_PATH = os.path.join(_HERE, "libgrape_b200.so")
 
 GL_LB = {"none": 0, "cm": 1, "wm": 2, "cta": 3, "strict": 4, "cmold": 5}
 APP = {"bfs": 0, "sssp": 1, "wcc": 2, "pagerank": 3, "cdlp": 4, "lcc": 5, "wcc_opt": 6,
-       "core_decomposition": 7, "kcore": 8, "kclique": 9}
+       "core_decomposition": 7, "kcore": 8, "kclique": 9, "bc": 10}
+# gl_bc_value: the reference's Output() line `oid c sigma depth` (c is an f32 value, widened exactly)
+BC_DTYPE = np.dtype([("centrality", "<f8"), ("path_num", "<f8"), ("depth", "<i8")])
 RESULT_DTYPE = {0: np.int64, 1: np.float64, 2: np.int64, 3: np.float64, 4: np.int64, 5: np.float64, 6: np.int64,
-                7: np.int64, 8: np.int64, 9: np.int64}
+                7: np.int64, 8: np.int64, 9: np.int64, 10: BC_DTYPE}
 GL_MAX_STEP_STATS = 512
 GL_IPC_HANDLE_BYTES = 64
 
@@ -454,7 +456,9 @@ class App:
     """One PIE app bound to a fragment (GPUWorker analogue).  "kcore" and "kclique"
     take their k as App("kcore", frag, k=...) (carried in max_round); it has no
     default.  The result of "kclique" is one Python int: the k-clique count of the
-    whole fragment group (result() takes no out array for it)."""
+    whole fragment group (result() takes no out array for it).  "bc" takes its
+    source as App("bc", frag, source_oid=...) and returns a BC_DTYPE record
+    (centrality, path_num, depth) per inner vertex."""
 
     def __init__(self, kind, frag, comm=None, **cfg):
         self.kind = APP[kind] if isinstance(kind, str) else kind

@@ -115,4 +115,5 @@ gl_app* make_wcc_opt();
 gl_app* make_core_decomposition();
 gl_app* make_kcore();
 gl_app* make_kclique();
+gl_app* make_bc();
 }  // namespace gl
