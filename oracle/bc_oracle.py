@@ -21,6 +21,11 @@ Two arithmetics:
 * mode="replay": the reference's one-thread order: sigma by sequential f64
   additions in (v ascending, row order), c as a running f32 sum in the same
   order (np.add.at on float32).  It reproduces the reference bit for bit.
+
+bc_rows() is the GPU app exactly: the same rules on the fragment's own CSR,
+with every sum taken in the order of the kernel's gathers.  The f64 mode
+differs from it only where a sum rounds (sigma past 2^53, or t values far
+apart in magnitude), which is why both are kept.
 """
 import numpy as np
 
@@ -123,4 +128,84 @@ def bc(n, src, dst, source, mode="f64"):
         v, u = _entries(rp, col, vs)
         keep = depth[u] == d - 1
         np.add.at(c, u[keep], t[v[keep]])   # float32 running sums in the reference's thread-0 order
+    return c, sigma, depth
+
+
+def warp_fold(a):
+    """The xor butterfly of warp_sum (engine.cuh) on the last axis (32 lanes): lane i += lane i ^ o for
+    o = 16, 8, 4, 2, 1.  Lanes i and i ^ o add the same two values, so every lane ends with lane 0's
+    value, which is a[:h] + a[h:] folded down to one."""
+    a = np.asarray(a, dtype=np.float64)
+    assert a.shape[-1] == 32
+    h = 16
+    while h:
+        a = a[..., :h] + a[..., h:]
+        h //= 2
+    return a[..., 0]
+
+
+def ordered_row_sums(rp, col, vs, term, short=32, chunk=1024):
+    """f64 sum of term[col[j]] over the row of every vertex in vs, in the order of the gathers of
+    app_bc.cu: a row of up to `short` entries is summed sequentially from 0.0; a longer row is cut into
+    `chunk`-entry chunks, lane l of a chunk sums the chunk's entries l, l + 32, .. sequentially, the 32
+    lane partials are folded by warp_fold, and the chunk sums are added in chunk order from 0.0.
+    short=None: one sequential sum over every row (k_bc_pull_multi / k_bc_back_multi).
+    term: f64 per vertex, 0.0 where an entry does not qualify (the kernels add 0.0 then too)."""
+    vs = np.asarray(vs, dtype=np.int64)
+    out = np.zeros(len(vs), dtype=np.float64)
+    if len(vs) == 0:
+        return out
+    deg = (rp[vs + 1] - rp[vs]).astype(np.int64)
+    total = int(deg.sum())
+    if total == 0:
+        return out
+    row = np.repeat(np.arange(len(vs), dtype=np.int64), deg)
+    first = np.concatenate([[0], np.cumsum(deg)[:-1]])
+    j = np.arange(total, dtype=np.int64) - np.repeat(first, deg)   # position within the row
+    vals = term[col[np.repeat(rp[vs].astype(np.int64), deg) + j].astype(np.int64)]
+    seq = np.ones(total, dtype=bool) if short is None else (deg <= short)[row]
+    # np.add.at is unbuffered: repeated indices are added one at a time, in entry order
+    np.add.at(out, row[seq], vals[seq])
+    lng = ~seq
+    if lng.any():
+        nch = (deg + chunk - 1) // chunk
+        nch[deg <= short] = 0
+        cbase = np.concatenate([[0], np.cumsum(nch)[:-1]])
+        ck = cbase[row[lng]] + j[lng] // chunk             # global chunk index, chunks in row / chunk order
+        lanes = np.zeros((int(nch.sum()), 32), dtype=np.float64)
+        np.add.at(lanes, (ck, (j[lng] % chunk) % 32), vals[lng])
+        np.add.at(out, np.repeat(np.arange(len(vs), dtype=np.int64), nch), warp_fold(lanes))
+    return out
+
+
+def bc_rows(n, rp, col, source, short=32, chunk=1024):
+    """What k_bc_fused computes, bit for bit, on the CSR (rp, col) in the kernel's own row order (global
+    vertex indices; a fragment's csr(0) when it is the only one).  Same rules as bc(): sigma(source) =
+    1, sigma = 1 at depth 1, the source keeps cacc, c = f32(f64(cacc) * sigma), t = f32((1 / sigma) *
+    (1 + f64(c))); every sum in the order of ordered_row_sums (short=None: the multi-fragment
+    kernels' sequential rows).  -> (c float32, sigma float64, depth int64)."""
+    rp = np.asarray(rp, dtype=np.int64)
+    col = np.asarray(col, dtype=np.int64)
+    levels, depth = levels_of(n, rp, col, source)
+    sigma = np.zeros(n, dtype=np.float64)
+    c = np.zeros(n, dtype=np.float32)
+    if not levels:
+        return c, sigma, depth
+    sigma[levels[0]] = 1.0
+    if len(levels) > 1:
+        sigma[levels[1]] = 1.0
+    for d in range(2, len(levels)):
+        term = np.where(depth == d - 1, sigma, 0.0)
+        sigma[levels[d]] = ordered_row_sums(rp, col, levels[d], term, short, chunk)
+    t = np.zeros(n, dtype=np.float32)
+    for d in range(len(levels) - 1, -1, -1):
+        vs = levels[d]
+        term = np.where(depth == d + 1, t.astype(np.float64), 0.0)
+        cacc = ordered_row_sums(rp, col, vs, term, short, chunk).astype(np.float32)
+        if d == 0:
+            c[vs] = cacc
+            break
+        cv = (cacc.astype(np.float64) * sigma[vs]).astype(np.float32)
+        c[vs] = cv
+        t[vs] = ((1.0 / sigma[vs]) * (1.0 + cv.astype(np.float64))).astype(np.float32)
     return c, sigma, depth

@@ -1,9 +1,9 @@
 """Betweenness centrality on the GPU (csrc/app_bc.cu): depth and sigma bit for
 bit against the digests of the reference CPU app (tests/golden/ref_bc_outputs.json)
-on every case of tests/bc_cases.py, c against the f64 oracle (oracle/bc_oracle.py)
-within (L + 1) * 2^-22 relative, where L is the deepest level; R-MAT 16 and 20
-against the oracle; repeated queries and push-only discovery bit-identical; and
-fragment groups (mgpu_bc_worker.py)."""
+on every case of tests/bc_cases.py, and depth, sigma and c bit for bit against
+the order-exact oracle (oracle/bc_oracle.py bc_rows) on the fragment's own CSR;
+R-MAT 16 and 20 the same way; repeated queries and push-only discovery
+bit-identical; and fragment groups (mgpu_bc_worker.py)."""
 import os
 import subprocess
 import sys
@@ -14,7 +14,8 @@ import pytest
 from oracle import bc_oracle as BO
 from tests import golden_io as G
 from tests import shapes as S
-from tests.bc_cases import as_indices, bc_cases, max_degree_index, ref_bc_outputs, source_index
+from tests.bc_cases import bc_cases, max_degree_index, ref_bc_outputs
+from tests.test_gpu_bc_shapes import check_exact
 from tests.util import pkg, rmat_graph
 
 pytestmark = pytest.mark.gpu
@@ -35,12 +36,10 @@ def run(frag, source, **cfg):
     return out, stats
 
 
-def check_c(got, c, depth):
-    reached = depth != BO.INF
-    L = int(depth[reached].max()) if reached.any() else 0
-    want = c.astype(np.float64)
-    assert np.all(np.abs(got - want) <= (L + 1) * 2.0 ** -22 * np.abs(want)), \
-        "c differs from the f64 oracle by more than (L + 1) 2^-22"
+def oracle_of(frag, source):
+    """bc_rows on the fragment's own CSR (lids are vertex indices in ascending-oid order)."""
+    rp, col, _ = frag.csr(0)
+    return BO.bc_rows(frag.ivnum, rp, col, frag.oid2lid(source))
 
 
 def check_stats(st, depth, launches=1):
@@ -64,16 +63,15 @@ def test_reference_digests(name):
     want = REF[name]
     frag = pkg().Fragment.from_edges(n, src, dst, None, oids=oids)
     got, st = run(frag, source)
-    s, d = as_indices(n, src, dst, oids)
-    c, sigma, depth = BO.bc(n, s, d, source_index(n, oids, source), "f64")
+    exact = oracle_of(frag, source)
+    depth = exact[2]
     assert G.digest(got["depth"]) == want["depth"]
     if name.startswith("diamond_chain"):
-        # past 2^53 a sum of path counts rounds: compare with the oracle's f64 arithmetic
-        assert np.all(np.abs(got["path_num"] - sigma) <= 1e-15 * sigma)
-        assert sigma.max() > 2.0 ** 53
+        # past 2^53 a sum of path counts rounds, and sigma is the kernel's order (check_exact below)
+        assert exact[1].max() > 2.0 ** 53
     else:
         assert G.digest(got["path_num"]) == want["sigma"]
-    check_c(got["centrality"], c, depth)
+    check_exact(got, exact)
     check_stats(st, depth)
     # a second query on another app object is bit-identical
     again, _ = run(frag, source)
@@ -81,27 +79,15 @@ def test_reference_digests(name):
     frag.close()
 
 
-_RMAT = {}
-
-
-def rmat_case(scale):
-    if scale not in _RMAT:
-        n, s, d, _ = rmat_graph(scale, seed=1)
-        source = max_degree_index(n, s, d)
-        _RMAT[scale] = (n, s, d, source, BO.bc(n, s, d, source, "f64"))
-    return _RMAT[scale]
-
-
 @pytest.mark.parametrize("scale", [16, 20])
 def test_rmat(scale):
-    n, s, d, source, (c, sigma, depth) = rmat_case(scale)
+    n, s, d, _ = rmat_graph(scale, seed=1)
+    source = max_degree_index(n, s, d)
     frag = pkg().Fragment.rmat(scale, 16, seed=1)
     app = pkg().App("bc", frag, source_oid=source)
     app.query()
     got = app.result()
-    assert np.array_equal(got["depth"], depth)
-    assert np.array_equal(got["path_num"], sigma)
-    check_c(got["centrality"], c, depth)
+    check_exact(got, oracle_of(frag, source))
     # two queries on one app are bit-identical
     app.query()
     assert app.result().tobytes() == got.tobytes()
@@ -153,3 +139,6 @@ def test_multi_fragment(nproc):
     runs = [l for l in p.stdout.splitlines() if l.startswith("[mgpu-bc] runs=")]
     assert runs, p.stdout[-4000:]
     assert p.stdout.count(" OK") == int(runs[-1].split("=")[1]) > 0
+    # the graphs whose sums round, a fan and long backward rows, each from at least its root and an absent oid
+    for name in ("order_chain", "back_chain", "fans", "kab33_2048"):
+        assert sum(l.startswith("[mgpu-bc] %s " % name) and l.endswith(" OK") for l in p.stdout.splitlines()) >= 2, name
