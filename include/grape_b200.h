@@ -493,6 +493,54 @@ typedef struct gl_app gl_app_t;
 int gl_app_create(gl_app_t** out, int kind, gl_frag_t* frag, gl_comm_t* comm,
                   const gl_app_config* cfg);
 
+/* Query statistics.  A superstep is one worker round; step 0 is PEval.  The k-th set of counters an
+ * app records (k = 0, 1, ...) is reported as step k + 1, also when PEval itself recorded it (CDLP's
+ * first round); a step nothing was recorded for reports zeros.  n_steps = min(supersteps,
+ * GL_MAX_STEP_STATS): only the per-step arrays are cut there; supersteps, entries_scanned,
+ * frontier_vertices and touched_vertices always cover the whole query, so the totals equal the sums
+ * of the step arrays whenever supersteps <= GL_MAX_STEP_STATS.  Exceptions, stated below: the
+ * one-fragment peels (n_steps = 1, totals only) and wcc_opt (step 0).  tests/test_gpu_stats.py holds
+ * the lines below on one fragment; on 2 and 3 fragments it holds the "several fragments" sentences.
+ *   BFS, fused or stepwise, any vertex order: step i >= 1 expands level i - 1; step_frontier =
+ *     the level's size, supersteps = levels + 1 (the last expansion finds nothing), frontier_vertices
+ *     = reached vertices, touched_vertices = vertices given a depth by an expansion (one fragment:
+ *     every reached vertex but the source).  A push step's step_entries is the row lengths of its
+ *     level, exactly.  A pull step (mode 1) reads rows of vertices not yet reached, in an order that
+ *     decides how far each row is read: at least one entry per vertex it finds, at most one probe of
+ *     the highest-degree neighbour plus the whole row per unreached vertex with a non-empty row.  A
+ *     source that is not in the graph: every counter 0 (supersteps 1 fused, 2 stepwise: the stepwise
+ *     query expands the empty frontier once).  A fused query keeps one record per level
+ *     for the first GL_MAX_STEP_STATS - 1 levels.
+ *     Several fragments, push steps: step_frontier and step_entries are this fragment's share (the
+ *     level's vertices it owns and their rows), so they add up to the one-fragment values over the
+ *     group; supersteps is the same on every rank, and one more than on one fragment (a closing step
+ *     of zeros) when the last level re-reported outer copies that were already visited; a push-only stepwise query sends 4 bytes per outer
+ *     vertex with an entry in the row of a reached inner vertex (a fragment learns that an outer vertex
+ *     is visited only by reaching it itself).  A pull step's step_frontier is not a share: the fused
+ *     query reports what the fragment found itself in the previous level, the stepwise query the whole
+ *     graph's level.  touched_vertices also counts the outer copies a fragment reaches.
+ *   PageRank (every variant), CDLP: each round is one step with step_frontier = ivnum, step_entries
+ *     = the CSR entries of the fragment, mode 2; touched_vertices = ivnum x rounds.  supersteps =
+ *     max_round + 2 (PageRank: PEval, the rounds, the round that stops) and max_round + 1 (CDLP: round
+ *     1 runs in PEval).  Several fragments: the same with this fragment's ivnum and entries.  CDLP's
+ *     step_entries is the size of the CSR its gather and sort are launched over, recorded by the host,
+ *     not counted by a kernel.
+ *   LCC, one fragment: step 1 counts the triangles: step_frontier = ivnum, step_entries = for every
+ *     entry (v, u) of the degree-ordered DAG, the length of u's DAG row; supersteps = 3.
+ *   core decomposition / k-core, one fragment: the whole peel is PEval's launch; supersteps counts its
+ *     sub-rounds while n_steps stays 1, so the counters are in the totals only: entries_scanned = the rows of the peeled
+ *     vertices (core decomposition: every entry), frontier_vertices = vertices peeled by a scan (k-core:
+ *     those with a result below k), touched_vertices = count updates (merged per warp, so it depends on
+ *     scheduling).
+ *   SSSP, WCC (label propagation): a vertex is expanded again whenever its value improves, in an
+ *     order threads race for, so the counts are bounded, not fixed: every reached vertex is expanded
+ *     at least once and, unless it keeps its initial value, written at least once.  SSSP's step 1 is
+ *     the source alone; WCC's step 1 expands every vertex; a dense WCC round (reserved[0] = 1, mode 2)
+ *     reports step_frontier = ivnum and the fragment's entries.
+ *   wcc_opt, one fragment: everything happens in PEval and is reported as step 0: step_frontier =
+ *     ivnum, step_entries = entries_scanned = 2 sampled entries per vertex + the rows scanned outside
+ *     the largest sampled component (which depends on the sampling's races); touched_vertices = ivnum.
+ *   BC, k-clique: see gl_bc_value and GL_KCLIQUE_MAX_K above. */
 #define GL_MAX_STEP_STATS 512
 typedef struct {
   int supersteps;            /* rounds executed (PEval counts as round 0)      */

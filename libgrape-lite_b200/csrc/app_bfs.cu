@@ -652,7 +652,8 @@ GL_DEV void bfs_list_pull(const PullArgs& a, const uint32_t* __restrict__ cur, u
 // Fused whole-query BFS (single fragment): ONE cooperative launch runs every
 // superstep.  Per-level device timestamps keep the ms/superstep report.
 // ---------------------------------------------------------------------------
-constexpr int kMaxFusedStats = 480;
+// level records a fused query keeps: with PEval's step 0 they fill the per-step arrays of gl_query_stats
+constexpr int kMaxFusedStats = GL_MAX_STEP_STATS - 1;
 struct BfsLevelStat {
   unsigned long long t_ns;
   unsigned long long scanned;
@@ -665,7 +666,9 @@ struct BfsFusedCtl {
   uint32_t has_src, src_lid;
   uint32_t overflow;   // ran out of level bitmaps
   uint32_t pad;
-  unsigned long long touched;
+  unsigned long long touched;   // of the whole query, over every level and launch
+  // entries scanned / vertices expanded by the levels past the level table below (it is finite)
+  unsigned long long over_scanned, over_frontier;
   unsigned long long t_begin;
   // state a relaunch starts from: parked by the kernel when it stops because
   // the level-bitmap ring is full (the host spills the finished levels and
@@ -761,6 +764,9 @@ GL_DEV void bfs_level_end(BfsFusedCtl* ctl, uint32_t depth_base, uint32_t depth,
     ls.frontier = (uint32_t) (frontier > 0xFFFFFFFFull ? 0xFFFFFFFFull : frontier);
     ls.mode = mode;
     ctl->stat[adepth] = ls;
+  } else {
+    ctl->over_scanned += VC->scanned;
+    ctl->over_frontier += frontier;
   }
   ctl->levels = adepth + 1;
   ctl->touched += VC->touched;
@@ -776,7 +782,7 @@ __global__ void k_bfs_seed_fused(uint32_t src, int has_src, uint32_t* lv0, uint3
   ctl->c[2] = ScanCtrl();
   ctl->levels = 0;
   ctl->overflow = 0;
-  ctl->touched = 0;
+  ctl->touched = ctl->over_scanned = ctl->over_frontier = 0;
   unsigned long long deg = 0;
   if (has_src) {
     lv0[src >> 5] |= 1u << (src & 31);
@@ -1546,9 +1552,10 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused_multi(BfsM
         ctl->xw[tl][1] = ctl->xt[1] - ctl->xt[0];
       }
       // the statistics record THIS fragment's share of the level's frontier (n_f is the whole graph's):
-      // what it found in the previous level (vertices that arrived as messages in a push level are not
-      // counted)
-      bfs_level_end(ctl, a.depth_base, depth, ctl->l_nf, phase == 1 ? 1u : 0u);
+      // a push level's is what its scan expanded; a pull level's is what the fragment found itself in
+      // the previous level (vertices that arrived as messages in a push level before it are not counted)
+      bfs_level_end(ctl, a.depth_base, depth, phase == 1 ? ctl->l_nf : ((const volatile ScanCtrl*) C)->frontier,
+                    phase == 1 ? 1u : 0u);
       ctl->l_nf = ((const volatile ScanCtrl*) C)->next_count;
       ctl->x_msg_rounds = msg_round - x.msg_round0;
       ctl->x_mirror_syncs = mseq - x.mirror_seq0;
@@ -2077,6 +2084,9 @@ struct BfsApp : gl_app {
     q_touched += h_ctl->touched;
     for (uint32_t i = 0; i < h_ctl->levels && i < (uint32_t) kMaxFusedStats; ++i)
       note_step(h_ctl->stat[i].scanned, h_ctl->stat[i].frontier, (int) h_ctl->stat[i].mode);
+    // a query deeper than the level table still reports all of its work
+    q_entries += h_ctl->over_scanned;
+    q_frontier += h_ctl->over_frontier;
     // every GPU left the kernel on the same all-reduced "frontier is empty": no round vote needed
     mm.decided_terminate = true;
     query_end = ev_done;
@@ -2086,9 +2096,8 @@ struct BfsApp : gl_app {
   // per-level device timestamps -> ms/superstep of the fused run
   void FillStats(gl_query_stats* st) override {
     if (!fused() || !h_ctl) return;
-    uint32_t L = std::min<uint32_t>(h_ctl->levels, (uint32_t) kMaxFusedStats);
-    st->supersteps = (int) L + 1;
-    int n = (int) std::min<uint32_t>(L + 1, GL_MAX_STEP_STATS);
+    st->supersteps = (int) h_ctl->levels + 1;
+    int n = (int) std::min<uint32_t>(h_ctl->levels, (uint32_t) kMaxFusedStats) + 1;
     st->n_steps = n;
     unsigned long long prev = h_ctl->t_begin;
     // PEval (seed) is part of the launch prologue.  One fragment: t_begin is the fused kernel's first
@@ -2203,7 +2212,9 @@ struct BfsApp : gl_app {
     pending_stats = false;
     if (rounds_noted) {
       const ScanCtrl& c = *eng.h_ctrl;   // mirrored by the vote kernel
-      note_step(c.scanned, (uint32_t) std::min<uint64_t>(n_f, 0xFFFFFFFFu), step_pull ? 1 : 0);
+      // this fragment's share of a push level is what its scan expanded; a pull step has no such
+      // count and reports the whole graph's level
+      note_step(c.scanned, (uint32_t) std::min<uint64_t>(step_pull ? n_f : c.frontier, 0xFFFFFFFFu), step_pull ? 1 : 0);
       q_touched += c.touched;
     }
     rounds_noted = true;

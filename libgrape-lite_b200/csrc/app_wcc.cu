@@ -187,7 +187,8 @@ struct WccApp : gl_app {
     GL_CUDA(cudaMemsetAsync(in_q, 0, sizeof(uint32_t) * words, s));
     GL_TRY(eng.fetch_ctrl());
     const ScanCtrl& c = *eng.h_ctrl;
-    note_step(c.scanned, (uint32_t) std::min<uint64_t>(c.frontier, 0xFFFFFFFFu), dense ? 2 : 0);
+    // a dense round sweeps every inner vertex (the sweep keeps no frontier count)
+    note_step(c.scanned, dense ? fv.ivnum : (uint32_t) std::min<uint64_t>(c.frontier, 0xFFFFFFFFu), dense ? 2 : 0);
     q_touched += c.touched;
     active_estimate = c.next_count;
     std::swap(out_local, in_q);
