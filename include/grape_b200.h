@@ -89,14 +89,15 @@ typedef struct {
   int edata_bytes;     /* 0 (EmptyType), 4 (float) or 8 (double)              */
   gl_csr_desc oe;      /* rows = ivnum (inner rows; outer rows are empty)     */
   gl_csr_desc ie;      /* directed: rows = ivnum; undirected: ignored         */
-  gl_csr_desc ov_ie;   /* optional reverse adjacency of OUTER vertices, rows =
-                          ovnum, cols = inner lids (what the reference keeps
-                          in ie_ rows ivnum..tvnum for kOnlyOut undirected,
-                          csr_edgecut_fragment_base.h:475-492); rows==0 -> the
-                          library derives it from oe                          */
+  gl_csr_desc ov_ie;   /* not read: gl_frag_create always derives the reverse
+                          adjacency of the OUTER vertices from oe (what the
+                          reference keeps in ie_ rows ivnum..tvnum for kOnlyOut
+                          undirected, csr_edgecut_fragment_base.h:475-492);
+                          gl_frag_copy_csr(which = 2) reads it back           */
   const uint32_t* ovgid;     /* gid of each outer vertex, ascending (IdParser
                                 format, grape/fragment/id_parser.h:28-55)     */
-  const int64_t* inner_oids; /* oid of each inner vertex, ascending; NULL ->
+  const int64_t* inner_oids; /* oid of each inner vertex in lid order, any
+                                order, no oid twice (GL_ERR_ARG); NULL ->
                                 oid = oid_base + lid                          */
   int64_t oid_base;
 } gl_frag_desc;
@@ -105,11 +106,14 @@ typedef struct {
  * Preconditions the library relies on (the reference's loaders satisfy them):
  *  - rows sorted by neighbour lid, inner neighbours first; ovgid ascending;
  *  - a DIRECTED fragment passes its in-edges in d->ie (without them BFS only pushes, PageRank pull
- *    falls back to push and WCC / wcc_opt are refused);
- *  - lids were assigned in ascending oid order inside each fragment and fids in ascending oid
- *    blocks IF the smallest-label tie-breaks of CDLP / WCC must equal the reference's smallest-OID
- *    rule (the apps tie-break on the smallest GID); with another vertex map attach a gl_vm_t
- *    (gl_app_set_vertex_map) to get oids back and expect ties to follow gid order. */
+ *    falls back to push and WCC / wcc_opt are refused).
+ * Any partition and any lid order are accepted.  Ties follow gid order: CDLP / WCC take the smallest
+ * GID as label and LCC orients equal degrees by gid (as the reference's lcc.h does; on repeated edges
+ * that decides the count).  The reference's vfile loader puts ascending oid blocks on the fids and
+ * assigns lids in oid order, so there the smallest gid is the smallest oid; its efile loader hashes
+ * oids to fids (oid % fnum) and assigns lids in order of first appearance, so there it is not.  With
+ * fnum > 1 attach a gl_vm_t (gl_app_set_vertex_map) to get WCC / CDLP labels back as oids (without one
+ * they are raw gids). */
 int gl_frag_create(gl_frag_t** out, const gl_frag_desc* d);
 /* HostFragment::PrepareToRunApp (host_fragment.h:122-215): split positions, outer ranges, the
  * reverse adjacency of the outer copies and the destination-fragment information are part of the

@@ -13,6 +13,7 @@
 #include <cub/cub.cuh>
 
 #include <algorithm>
+#include <functional>
 
 #include "dense.cuh"
 #include "fragment.h"
@@ -810,6 +811,23 @@ int gl_frag_create(gl_frag_t** out, const gl_frag_desc* d) {
   }
   if (d->inner_oids && d->ivnum) {
     f->h_inner_oids.assign(d->inner_oids, d->inner_oids + d->ivnum);
+    // inner_oids is in lid order, whatever order the host assigned lids in (the reference's edge-file
+    // loader numbers vertices by first appearance): oid -> lid then goes through a sorted side index
+    const auto& io = f->h_inner_oids;
+    if (std::adjacent_find(io.begin(), io.end(), std::greater_equal<int64_t>()) != io.end()) {
+      f->h_oid_index.resize(d->ivnum);
+      for (uint32_t l = 0; l < d->ivnum; ++l) f->h_oid_index[l] = {io[l], l};
+      std::sort(f->h_oid_index.begin(), f->h_oid_index.end());
+      auto dup = std::adjacent_find(f->h_oid_index.begin(), f->h_oid_index.end(),
+                                    [](const std::pair<int64_t, uint32_t>& a, const std::pair<int64_t, uint32_t>& b) {
+                                      return a.first == b.first;
+                                    });
+      if (dup != f->h_oid_index.end()) {
+        set_error("inner oid %lld appears twice (lids %u and %u)", (long long) dup->first, dup->second,
+                  (dup + 1)->second);
+        return fail(GL_ERR_ARG);
+      }
+    }
     if (cudaMalloc(&f->inner_oids, sizeof(int64_t) * d->ivnum) != cudaSuccess ||
         cudaMemcpy(f->inner_oids, d->inner_oids, sizeof(int64_t) * d->ivnum, cudaMemcpyHostToDevice) != cudaSuccess) {
       set_error("inner oid upload failed");
@@ -876,6 +894,15 @@ int gl_frag_copy_ovgid(const gl_frag_t* f, uint32_t* ovgid) {
 
 int gl_frag_oid2lid(const gl_frag_t* f, int64_t oid, uint32_t* lid) {
   GL_ARG(f && lid, "null argument");
+  if (!f->h_oid_index.empty()) {
+    auto it = std::lower_bound(f->h_oid_index.begin(), f->h_oid_index.end(), std::make_pair(oid, 0u));
+    if (it == f->h_oid_index.end() || it->first != oid) {
+      set_error("oid %lld is not an inner vertex of fragment %u", (long long) oid, f->fid);
+      return GL_ERR_ARG;
+    }
+    *lid = it->second;
+    return GL_OK;
+  }
   if (!f->h_inner_oids.empty()) {
     auto it = std::lower_bound(f->h_inner_oids.begin(), f->h_inner_oids.end(), oid);
     if (it == f->h_inner_oids.end() || *it != oid) {

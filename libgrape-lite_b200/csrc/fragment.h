@@ -3,6 +3,7 @@
 // (grape/cuda/fragment/host_fragment.h, device_fragment.h) with an SoA CSR:
 // 64-bit row pointers, 32-bit neighbour lids, separate weight array.
 #pragma once
+#include <utility>
 #include <vector>
 
 #include "common.cuh"
@@ -32,7 +33,10 @@ struct gl_frag {
   uint32_t* outer_range = nullptr;  // device [fnum+1]
   std::vector<uint32_t> h_outer_range;
   int64_t* inner_oids = nullptr;    // device or null
-  std::vector<int64_t> h_inner_oids;
+  std::vector<int64_t> h_inner_oids;   // lid order
+  // (oid, lid) sorted by oid when h_inner_oids is not ascending; empty when it is (gl_frag_oid2lid
+  // then searches h_inner_oids itself)
+  std::vector<std::pair<int64_t, uint32_t>> h_oid_index;
   int64_t oid_base = 0;
   uint64_t part_chunk = 0;  // ceil(n/fnum) of the segmented partitioner (0 = unknown)
   // bitmap of inner vertices with out-degree > 0 (pull candidates)
