@@ -408,9 +408,32 @@ typedef enum {
                           endpoint survives the k-core peel (k = max_round);
                           v is in the k-core iff value >= k                   */
   GL_APP_KCLIQUE = 9,  /* kclique/kclique.h (--kclique_k = max_round), see below */
-  GL_APP_BC = 10       /* bc/staged_bc_bfs.h + bc/staged_bc.h (--bc_source =
+  GL_APP_BC = 10,      /* bc/staged_bc_bfs.h + bc/staged_bc.h (--bc_source =
                           source_oid)  result: gl_bc_value, see below          */
+  GL_APP_LCC_DIRECTED = 11  /* lcc/lcc_directed.h (LCCDirected)  result: double,
+                               see below                                        */
 } gl_app_kind;
+
+/* GL_APP_LCC_DIRECTED: the local clustering coefficient of a directed graph (the reference's
+ * run_app_opt --application lcc --directed), one double per inner vertex in lid order.  It needs a
+ * directed fragment with its in-edges (gl_frag_desc.ie / kBothOutIn): an undirected fragment (use
+ * GL_APP_LCC there) and a directed one without ie are refused at gl_app_create with GL_ERR_ARG.  Edge
+ * data is ignored.  For an inner vertex v, over its out-row and in-row together, oe(v) + ie(v), with
+ * multiplicity:
+ *   N(v) = the distinct neighbours in the union (v itself when v has a self loop);
+ *   d(v) = |N(v)|, the deduplicated degree;
+ *   w(v,u) = the CSR entries of u in oe(v) + ie(v) = #(v->u) + #(u->v) (symmetric);
+ *   tri(v) = the sum of w(u,x) over unordered pairs {u, x} of N(v) \ {v}, u != x, u and x adjacent;
+ *   lcc(v) = double(tri(v)) / double(int64(d) * (d - 1)); 0.0 when d < 2.
+ * Each triangle is counted once along a degree orientation (|oe| + |ie| entries); the reference breaks
+ * degree ties by IdHasher(gid), this app by gid.  Every weight is symmetric, so any strict total order
+ * gives the same tri.  Two deliberate differences from the reference:
+ *   - weights are exact: the reference keeps w in a uint8_t, so a pair joined by 256 entries weighs 0
+ *     there (and 300 entries weigh 44); here w is exact below 2^32 entries per pair;
+ *   - tri is counted in 64 bits: the reference's LCCDirected32, which it picks for graphs of at most
+ *     2^32 edges, can wrap on hubs.
+ * Where every pair has fewer than 256 entries and the counts fit 32 bits, the result equals the
+ * reference's bit for bit. */
 
 /* GL_APP_BC: single-source betweenness centrality, one gl_bc_value per inner vertex in lid order: the
  * reference's Output() line `oid c sigma depth` (gl_app_result_oids gives the oid).  A directed fragment
@@ -531,6 +554,11 @@ int gl_app_create(gl_app_t** out, int kind, gl_frag_t* frag, gl_comm_t* comm,
  *     not counted by a kernel.
  *   LCC, one fragment: step 1 counts the triangles: step_frontier = ivnum, step_entries = for every
  *     entry (v, u) of the degree-ordered DAG, the length of u's DAG row; supersteps = 3.
+ *   LCC_DIRECTED: step 1 counts the triangles (mode 2): step_frontier = ivnum, step_entries = for every
+ *     oriented entry (v, u), the length of u's oriented row N+(u); supersteps = 3; entries_scanned and
+ *     frontier_vertices carry the same values, touched_vertices = ivnum.  Several fragments: the same
+ *     with this fragment's ivnum and the oriented entries of its inner vertices, so the shares add up to
+ *     the one-fragment values over the group.
  *   core decomposition / k-core, one fragment: the whole peel is PEval's launch; supersteps counts its
  *     sub-rounds while n_steps stays 1, so the counters are in the totals only: entries_scanned = the rows of the peeled
  *     vertices (core decomposition: every entry), frontier_vertices = vertices peeled by a scan (k-core:

@@ -34,14 +34,15 @@ struct Engine {
 // fragment of the group: CUDA IPC export, one blob exchange, bulk peer copies, then a peer barrier so no
 // fragment changes its arrays while a peer still reads them.  Collective when fnum > 1.  The device
 // tables d_rp / d_col [fnum] point at the replicas and, at [fid], at this fragment's own arrays (which
-// must be whole cudaMalloc allocations).
+// must be whole cudaMalloc allocations).  An optional per-entry weight array w travels the same way
+// (d_w [fnum]; left unallocated when w is null).
 struct PeerCsr {
   std::vector<DevBuf<uint64_t>> rep_rp;
-  std::vector<DevBuf<uint32_t>> rep_col;
+  std::vector<DevBuf<uint32_t>> rep_col, rep_w;
   DevBuf<const uint64_t*> d_rp;
-  DevBuf<const uint32_t*> d_col;
+  DevBuf<const uint32_t*> d_col, d_w;
   int replicate(MessageManager& mm, cudaStream_t s, const gl_frag_view& fv, const uint64_t* rp,
-                const uint32_t* col, uint64_t m);
+                const uint32_t* col, uint64_t m, const uint32_t* w = nullptr);
 };
 
 struct StepRecorder {
@@ -111,6 +112,7 @@ gl_app* make_wcc();
 gl_app* make_pagerank();
 gl_app* make_cdlp();
 gl_app* make_lcc();
+gl_app* make_lcc_directed();
 gl_app* make_wcc_opt();
 gl_app* make_core_decomposition();
 gl_app* make_kcore();

@@ -621,30 +621,35 @@ int MessageManager::AllReduceF64(double* v, int n, int op) {
 namespace {
 // what a fragment tells its peers about its CSR part
 struct PeerCsrExport {
-  cudaIpcMemHandle_t h_rp, h_col;
+  cudaIpcMemHandle_t h_rp, h_col, h_w;
   uint64_t rows, m;
 };
 }  // namespace
 
 int PeerCsr::replicate(MessageManager& mm, cudaStream_t s, const gl_frag_view& fv, const uint64_t* rp,
-                       const uint32_t* col, uint64_t m) {
+                       const uint32_t* col, uint64_t m, const uint32_t* w) {
   if (!d_rp) {
     GL_CUDA(d_rp.alloc(fv.fnum));
     GL_CUDA(d_col.alloc(fv.fnum));
   }
+  if (w && !d_w) GL_CUDA(d_w.alloc(fv.fnum));
   rep_rp.clear();
   rep_col.clear();
+  rep_w.clear();
   rep_rp.resize(fv.fnum);
   rep_col.resize(fv.fnum);
+  rep_w.resize(fv.fnum);
   std::vector<const uint64_t*> r_rp(fv.fnum);
-  std::vector<const uint32_t*> r_col(fv.fnum);
+  std::vector<const uint32_t*> r_col(fv.fnum), r_w(fv.fnum);
   r_rp[fv.fid] = rp;
   r_col[fv.fid] = col;
+  r_w[fv.fid] = w;
   if (fv.fnum > 1) {
     PeerCsrExport mine;
     memset(&mine, 0, sizeof(mine));
     GL_CUDA(cudaIpcGetMemHandle(&mine.h_rp, (void*) rp));
     GL_CUDA(cudaIpcGetMemHandle(&mine.h_col, (void*) col));
+    if (w) GL_CUDA(cudaIpcGetMemHandle(&mine.h_w, (void*) w));
     mine.rows = fv.ivnum;
     mine.m = m;
     std::vector<char> all;
@@ -656,18 +661,26 @@ int PeerCsr::replicate(MessageManager& mm, cudaStream_t s, const gl_frag_view& f
       GL_CUDA(rep_col[g].alloc(std::max<uint64_t>(ex.m, 4)));
       r_rp[g] = rep_rp[g];
       r_col[g] = rep_col[g];
-      void *p_rp = nullptr, *p_col = nullptr;
+      void *p_rp = nullptr, *p_col = nullptr, *p_w = nullptr;
       GL_CUDA(cudaIpcOpenMemHandle(&p_rp, ex.h_rp, cudaIpcMemLazyEnablePeerAccess));
       GL_CUDA(cudaIpcOpenMemHandle(&p_col, ex.h_col, cudaIpcMemLazyEnablePeerAccess));
       GL_CUDA(cudaMemcpyAsync(rep_rp[g], p_rp, sizeof(uint64_t) * (ex.rows + 1), cudaMemcpyDeviceToDevice, s));
       if (ex.m) GL_CUDA(cudaMemcpyAsync(rep_col[g], p_col, sizeof(uint32_t) * ex.m, cudaMemcpyDeviceToDevice, s));
+      if (w) {
+        GL_CUDA(rep_w[g].alloc(std::max<uint64_t>(ex.m, 4)));
+        r_w[g] = rep_w[g];
+        GL_CUDA(cudaIpcOpenMemHandle(&p_w, ex.h_w, cudaIpcMemLazyEnablePeerAccess));
+        if (ex.m) GL_CUDA(cudaMemcpyAsync(rep_w[g], p_w, sizeof(uint32_t) * ex.m, cudaMemcpyDeviceToDevice, s));
+      }
       GL_CUDA(cudaStreamSynchronize(s));
       GL_CUDA(cudaIpcCloseMemHandle(p_rp));
       GL_CUDA(cudaIpcCloseMemHandle(p_col));
+      if (p_w) GL_CUDA(cudaIpcCloseMemHandle(p_w));
     }
   }
   GL_CUDA(cudaMemcpyAsync(d_rp, r_rp.data(), sizeof(void*) * fv.fnum, cudaMemcpyHostToDevice, s));
   GL_CUDA(cudaMemcpyAsync(d_col, r_col.data(), sizeof(void*) * fv.fnum, cudaMemcpyHostToDevice, s));
+  if (w) GL_CUDA(cudaMemcpyAsync(d_w, r_w.data(), sizeof(void*) * fv.fnum, cudaMemcpyHostToDevice, s));
   GL_CUDA(cudaStreamSynchronize(s));
   if (fv.fnum > 1) GL_TRY(mm.PeerBarrier(s));   // every peer has finished reading my arrays
   return GL_OK;

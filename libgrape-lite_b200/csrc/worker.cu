@@ -122,6 +122,7 @@ int gl_app_create(gl_app_t** out, int kind, gl_frag_t* frag, gl_comm_t* comm,
     case GL_APP_KCORE: a = make_kcore(); break;
     case GL_APP_KCLIQUE: a = make_kclique(); break;
     case GL_APP_BC: a = make_bc(); break;
+    case GL_APP_LCC_DIRECTED: a = make_lcc_directed(); break;
     default:
       set_error("unknown app kind %d", kind);
       return GL_ERR_ARG;
