@@ -274,7 +274,10 @@ typedef struct {
                                 BatchShuffleMessageManager::SyncInnerVertices,
                                 grape/cuda/parallel/batch_shuffle_message_manager.h:142-220);
                                 0 = 8 bytes per inner vertex of the largest fragment
-                                is NOT assumed: pass it explicitly                */
+                                is NOT assumed: pass it explicitly.
+                                GL_APP_PAGERANK_VC on F > 1 vertex-cut fragments
+                                needs mirror_bytes >= 8 * ceil(n_vertices / F)
+                                (gl_comm_create rounds it up to a multiple of 256) */
 } gl_comm_desc;
 #define GL_IPC_HANDLE_BYTES 64
 int gl_comm_create(gl_comm_t** out, const gl_comm_desc* d);
@@ -410,9 +413,85 @@ typedef enum {
   GL_APP_KCLIQUE = 9,  /* kclique/kclique.h (--kclique_k = max_round), see below */
   GL_APP_BC = 10,      /* bc/staged_bc_bfs.h + bc/staged_bc.h (--bc_source =
                           source_oid)  result: gl_bc_value, see below          */
-  GL_APP_LCC_DIRECTED = 11  /* lcc/lcc_directed.h (LCCDirected)  result: double,
-                               see below                                        */
+  GL_APP_LCC_DIRECTED = 11,  /* lcc/lcc_directed.h (LCCDirected)  result: double,
+                                see below                                        */
+  GL_APP_PAGERANK_VC = 12   /* pagerank/pagerank_vc.h (PageRankVC, run_app --vc) on a
+                               gl_vcfrag_t: created by gl_vc_app_create only;
+                               result: double per master vertex, see below      */
 } gl_app_kind;
+
+/* ------------------------------------------------------------------ *
+ * Vertex-cut fragment: replaces ImmutableVertexcutFragment with the 2-D
+ * VCPartitioner (grape/fragment/immutable_vertexcut_fragment.h,
+ * grape/vertex_map/partitioner.h).  Vertices are the oids 0..n-1, F = fnum
+ * must be a perfect square, s = sqrt(F):
+ *   mvc = ceil(n / F), vchunk = mvc * s;
+ *   edge (a, b) belongs to fragment (a / vchunk) * s + b / vchunk;
+ *   the masters of fragment f are [f * mvc, min((f + 1) * mvc, n)) (tail
+ *   fragments may have none);
+ *   the source range of f is chunk f / s, the destination range chunk f % s
+ *   (chunk c = [c * vchunk, min((c + 1) * vchunk, n))); the masters lie in the
+ *   source range.  The local vertices are the union of the two ranges, lower
+ *   chunk first, each in oid order (one range on a diagonal block).
+ * The device holds a local CSR over the local vertices: every block edge
+ * (a, b) puts b in a's row and a in b's row (a self loop twice in its row,
+ * duplicates kept), 64-bit row pointers, 32-bit local column ids, rows sorted.
+ * ------------------------------------------------------------------ */
+typedef struct gl_vcfrag gl_vcfrag_t;
+typedef struct {
+  uint64_t n_vertices;
+  uint64_t n_edges;
+  const int64_t* src;  /* host pointers; any superset of this fid's block (e.g.
+                          the whole edge list): edges of other blocks are ignored */
+  const int64_t* dst;
+  uint32_t fid, fnum;
+} gl_vcfrag_desc;
+/* GL_ERR_ARG: fnum not a perfect square, fid >= fnum, an endpoint of ANY edge
+ * outside [0, n), or 2^32 or more local vertices. */
+int gl_vcfrag_create(gl_vcfrag_t** out, const gl_vcfrag_desc* d);
+/* The device R-MAT generator of gl_frag_build_rmat (ids in [0, 2^scale)); every
+ * generated edge is used once, as generated (the app treats each edge both ways).
+ * weight_mode is ignored. */
+int gl_vcfrag_build_rmat(gl_vcfrag_t** out, const gl_rmat_desc* d);
+typedef struct {
+  uint32_t fid, fnum;
+  uint64_t n_vertices;
+  uint64_t master_begin, master_end;  /* oids [begin, end)                            */
+  uint64_t src_begin, src_end;        /* source range (chunk fid / s)                  */
+  uint64_t dst_begin, dst_end;        /* destination range (chunk fid % s)             */
+  uint64_t local_vnum;                /* |source range U destination range|            */
+  uint64_t block_edges;               /* edges of this fragment's block                 */
+  uint64_t entries;                   /* local CSR entries = 2 * block_edges            */
+  uint64_t device_bytes;              /* HBM held by the fragment                      */
+} gl_vcfrag_info;
+int gl_vcfrag_get_info(const gl_vcfrag_t*, gl_vcfrag_info* out);
+void gl_vcfrag_destroy(gl_vcfrag_t*);
+
+/* GL_APP_PAGERANK_VC: PageRankVC on a vertex-cut fragment.  Uses pr_delta (d) and max_round (R);
+ * every other gl_app_config field is ignored.  gl_app_create refuses kind 12 and gl_vc_app_create
+ * every other kind (GL_ERR_ARG); gl_app_set_vertex_map is refused (GL_ERR_ARG).  The result is one
+ * double per master vertex in oid order (gl_app_result_oids gives the master oids).  With F > 1 the
+ * app needs an opened communicator with mirror_bytes >= 8 * mvc (GL_ERR_ARG otherwise); F = 1 does
+ * no communication and comm may be NULL.
+ * Semantics (n vertices, deg(v) = edge endpoints equal to v: a self loop counts twice, every duplicate
+ * counts; v is dangling when deg(v) = 0; D = dangling vertices of the whole graph):
+ *   R <= 0: nothing runs, every result is 0.0, supersteps = 1.
+ *   PEval: p = 1/n; mr[v] = p if v is dangling, else p / deg(v); dangling_sum = p * D; curr = mr
+ *          on every local copy.
+ *   IncEval step k = 1..R: base = (1 - d)/n + d * dangling_sum / n, then dangling_sum = base * D;
+ *          next[v] = sum of curr[u] over the local CSR entries (v, u); sum(v) = the partial next[v]
+ *          of every fragment holding v, folded in fid order; k < R: mr[v] = (base + d * sum) / deg(v)
+ *          (base when dangling) and curr = mr on every copy; k = R: result[v] = sum * d + base.
+ *   Everything is f64 and every sum has a fixed order (a row's entries in fixed per-lane strides and
+ *   shuffle tree, long rows in fixed 4096-entry chunks folded in order), so the same input gives
+ *   bit-identical output on every run.  It equals GL_APP_PAGERANK (push or pull, same d and R) on
+ *   the undirected edge-cut fragment of the same edges up to f64 summation order.
+ * Stats: supersteps = R + 1; step k = round k (1..R), mode 2, step_frontier = local vertices,
+ *   step_entries = local CSR entries (2 x block edges, a host count); touched_vertices = masters x R.
+ *   msg_bytes_sent (F > 1) = (R + 1) x G + R x S where G = 8 |masters(g)| summed over the other
+ *   fragments g whose masters lie in this fragment's local range (the gather of PEval's degrees and
+ *   of every round's sums) and S = 8 |own masters| x (the other fragments holding them) (the scatter
+ *   of PEval and of rounds 1..R-1).  R <= 0: 0. */
 
 /* GL_APP_LCC_DIRECTED: the local clustering coefficient of a directed graph (the reference's
  * run_app_opt --application lcc --directed), one double per inner vertex in lid order.  It needs a
@@ -519,6 +598,10 @@ typedef struct gl_app gl_app_t;
 /* GPUWorker::Init: PrepareToRunApp + context Init (gpu_worker.h:44-65) */
 int gl_app_create(gl_app_t** out, int kind, gl_frag_t* frag, gl_comm_t* comm,
                   const gl_app_config* cfg);
+/* Apps on a vertex-cut fragment (GL_APP_PAGERANK_VC only, see above); the handle is used with
+ * gl_app_query / gl_app_result / gl_app_result_oids / gl_app_destroy like any other app. */
+int gl_vc_app_create(gl_app_t** out, int kind, gl_vcfrag_t* frag, gl_comm_t* comm,
+                     const gl_app_config* cfg);
 
 /* Query statistics.  A superstep is one worker round; step 0 is PEval.  The k-th set of counters an
  * app records (k = 0, 1, ...) is reported as step k + 1, also when PEval itself recorded it (CDLP's

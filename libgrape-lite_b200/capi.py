@@ -11,11 +11,11 @@ LIB_PATH = os.path.join(_HERE, "libgrape_b200.so")
 GL_LB = {"none": 0, "cm": 1, "wm": 2, "cta": 3, "strict": 4, "cmold": 5}
 APP = {"bfs": 0, "sssp": 1, "wcc": 2, "pagerank": 3, "cdlp": 4, "lcc": 5, "wcc_opt": 6,
        "core_decomposition": 7, "kcore": 8, "kclique": 9, "bc": 10,
-       "lcc_directed": 11}
+       "lcc_directed": 11, "pagerank_vc": 12}
 # gl_bc_value: the reference's Output() line `oid c sigma depth` (c is an f32 value, widened exactly)
 BC_DTYPE = np.dtype([("centrality", "<f8"), ("path_num", "<f8"), ("depth", "<i8")])
 RESULT_DTYPE = {0: np.int64, 1: np.float64, 2: np.int64, 3: np.float64, 4: np.int64, 5: np.float64, 6: np.int64,
-                7: np.int64, 8: np.int64, 9: np.int64, 10: BC_DTYPE, 11: np.float64}
+                7: np.int64, 8: np.int64, 9: np.int64, 10: BC_DTYPE, 11: np.float64, 12: np.float64}
 GL_MAX_STEP_STATS = 512
 GL_IPC_HANDLE_BYTES = 64
 
@@ -51,6 +51,19 @@ class FragInfo(C.Structure):
                 ("total_vnum", C.c_uint64), ("oe_num", C.c_uint64), ("ie_num", C.c_uint64),
                 ("directed", C.c_int), ("load_strategy", C.c_int), ("edata_bytes", C.c_int),
                 ("fid_offset", C.c_int), ("device_bytes", C.c_uint64), ("max_degree", C.c_uint32)]
+
+
+class VcFragDesc(C.Structure):
+    _fields_ = [("n_vertices", C.c_uint64), ("n_edges", C.c_uint64), ("src", C.c_void_p), ("dst", C.c_void_p),
+                ("fid", C.c_uint32), ("fnum", C.c_uint32)]
+
+
+class VcFragInfo(C.Structure):
+    _fields_ = [("fid", C.c_uint32), ("fnum", C.c_uint32), ("n_vertices", C.c_uint64),
+                ("master_begin", C.c_uint64), ("master_end", C.c_uint64), ("src_begin", C.c_uint64),
+                ("src_end", C.c_uint64), ("dst_begin", C.c_uint64), ("dst_end", C.c_uint64),
+                ("local_vnum", C.c_uint64), ("block_edges", C.c_uint64), ("entries", C.c_uint64),
+                ("device_bytes", C.c_uint64)]
 
 
 class AppConfig(C.Structure):
@@ -98,7 +111,8 @@ SYMBOLS = [
     "gl_varray_h2d", "gl_varray_d2h", "gl_varray_destroy", "gl_app_config_default", "gl_app_create", "gl_app_query", "gl_app_result",
     "gl_app_result_oids", "gl_app_destroy", "gl_edge_scan_queue", "gl_compact_bitmap", "gl_dev_alloc",
     "gl_dev_free", "gl_dev_memset", "gl_dev_h2d", "gl_dev_d2h", "gl_dev_sync", "gl_kernel_launch_count",
-    "gl_host_alloc_pinned", "gl_host_free_pinned",
+    "gl_host_alloc_pinned", "gl_host_free_pinned", "gl_vcfrag_create", "gl_vcfrag_build_rmat",
+    "gl_vcfrag_get_info", "gl_vcfrag_destroy", "gl_vc_app_create",
 ]
 
 
@@ -120,7 +134,8 @@ def lib():
         L.gl_mm_destroy.restype = None
         L.gl_vm_destroy.restype = None
         L.gl_queue_destroy.restype = None
-        for f in ("gl_frag_destroy", "gl_comm_destroy", "gl_app_destroy", "gl_app_config_default"):
+        for f in ("gl_frag_destroy", "gl_comm_destroy", "gl_app_destroy", "gl_app_config_default",
+                  "gl_vcfrag_destroy"):
             getattr(L, f).restype = None
         _LIB = L
     return _LIB
@@ -281,6 +296,44 @@ class Fragment:
     def close(self):
         if self.h:
             lib().gl_frag_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        if getattr(self, "h", None) and _LIB is not None:
+            self.close()
+
+
+class VcFragment:
+    """Device-resident vertex-cut fragment (ImmutableVertexcutFragment with the 2-D VCPartitioner):
+    fnum must be a perfect square; every rank may pass the whole edge list."""
+
+    def __init__(self, handle):
+        self.h = handle
+        info = VcFragInfo()
+        check(lib().gl_vcfrag_get_info(self.h, C.byref(info)))
+        self.info = {k: getattr(info, k) for k, _ in VcFragInfo._fields_}
+        self.fid, self.fnum = info.fid, info.fnum
+        self.n_masters = info.master_end - info.master_begin
+
+    @classmethod
+    def from_edges(cls, n_vertices, src, dst, fid=0, fnum=1):
+        src = np.ascontiguousarray(src, dtype=np.int64)
+        dst = np.ascontiguousarray(dst, dtype=np.int64)
+        d = VcFragDesc(n_vertices, len(src), _p(src), _p(dst), fid, fnum)
+        h = C.c_void_p()
+        check(lib().gl_vcfrag_create(C.byref(h), C.byref(d)))
+        return cls(h)
+
+    @classmethod
+    def rmat(cls, scale, edgefactor=16, seed=1, fid=0, fnum=1):
+        d = RmatDesc(scale, edgefactor, seed, 0, fid, fnum)
+        h = C.c_void_p()
+        check(lib().gl_vcfrag_build_rmat(C.byref(h), C.byref(d)))
+        return cls(h)
+
+    def close(self):
+        if self.h:
+            lib().gl_vcfrag_destroy(self.h)
             self.h = None
 
     def __del__(self):
@@ -459,7 +512,8 @@ class App:
     default.  The result of "kclique" is one Python int: the k-clique count of the
     whole fragment group (result() takes no out array for it).  "bc" takes its
     source as App("bc", frag, source_oid=...) and returns a BC_DTYPE record
-    (centrality, path_num, depth) per inner vertex."""
+    (centrality, path_num, depth) per inner vertex.  A VcFragment takes "pagerank_vc"
+    (gl_vc_app_create); its result is one double per master vertex."""
 
     def __init__(self, kind, frag, comm=None, **cfg):
         self.kind = APP[kind] if isinstance(kind, str) else kind
@@ -483,7 +537,8 @@ class App:
             setattr(c, k, v)
         self.cfg = c
         self.h = C.c_void_p()
-        check(lib().gl_app_create(C.byref(self.h), self.kind, frag.h, comm.h if comm else None, C.byref(c)))
+        create = lib().gl_vc_app_create if isinstance(frag, VcFragment) else lib().gl_app_create
+        check(create(C.byref(self.h), self.kind, frag.h, comm.h if comm else None, C.byref(c)))
         self.stats = QueryStats()
 
     def set_vertex_map(self, vm):
@@ -503,12 +558,15 @@ class App:
             check(lib().gl_app_result(self.h, _p(one), one.nbytes))
             return int(one.view(np.uint64)[0])   # the uint64 count (modulo 2^64)
         if out is None:
-            out = np.empty(self.frag.ivnum, dtype=dt)
+            out = np.empty(self._count(), dtype=dt)
         check(lib().gl_app_result(self.h, _p(out), out.nbytes))
         return out
 
+    def _count(self):
+        return self.frag.n_masters if isinstance(self.frag, VcFragment) else self.frag.ivnum
+
     def result_oids(self):
-        out = np.empty(self.frag.ivnum, dtype=np.int64)
+        out = np.empty(self._count(), dtype=np.int64)
         check(lib().gl_app_result_oids(self.h, _p(out), len(out)))
         return out
 

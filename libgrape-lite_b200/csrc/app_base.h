@@ -58,6 +58,8 @@ struct StepRecorder {
 
 }  // namespace gl
 
+struct gl_vcfrag;
+
 struct gl_app {
   int kind = 0;
   gl_frag* frag = nullptr;
@@ -80,6 +82,7 @@ struct gl_app {
   virtual int Result(void* host_out, size_t bytes) = 0;
   virtual size_t ResultElemBytes() const = 0;
   virtual size_t ResultCount() const { return frag ? frag->ivnum : 0; }   // elements gl_app_result writes
+  virtual int ResultOids(int64_t* host_out, size_t count);               // gl_app_result_oids (worker.cu)
   virtual void FillStats(gl_query_stats*) {}   // apps that time supersteps on the device
   virtual void AfterRound() {}                 // runs after every FinishARound (global round statistics)
   // Apps whose whole query is one launch record this event in-stream right after the query's last
@@ -118,4 +121,5 @@ gl_app* make_core_decomposition();
 gl_app* make_kcore();
 gl_app* make_kclique();
 gl_app* make_bc();
+gl_app* make_pagerank_vc(gl_vcfrag* f);
 }  // namespace gl

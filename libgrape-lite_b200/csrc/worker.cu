@@ -1,6 +1,7 @@
 // worker.cu — engine bookkeeping and the PIE worker loop behind the C ABI.
 // Replaces grape::cuda::GPUWorker::{Init,Query} (grape/cuda/worker/gpu_worker.h:44-107).
 #include "apps_common.cuh"
+#include "vcfrag.h"
 
 namespace gl {
 
@@ -15,7 +16,7 @@ int Engine::init(const gl_frag* f) {
   GL_CUDA(h_ctrl.alloc(1));
   memset(h_ctrl, 0, sizeof(ScanCtrl));
   // every hub row has > hub_deg entries, so (#pieces) <= M/kHubChunk + M/hub_deg
-  uint64_t m = std::max<uint64_t>(f->oe.entries, f->ie.entries);
+  uint64_t m = f ? std::max<uint64_t>(f->oe.entries, f->ie.entries) : 0;   // null: an app on a vertex-cut fragment
   uint64_t cap = m / kHubChunk + m / std::max<uint32_t>(hub_deg, 1) + 1024;
   hub_cap = (uint32_t) std::min<uint64_t>(cap, 0x7FFFFFFFull);
   GL_CUDA(hubs.alloc(hub_cap));
@@ -79,6 +80,7 @@ extern "C" {
 
 int gl_app_set_vertex_map(gl_app_t* a, const gl_vm_t* vm) {
   GL_ARG(a, "null argument");
+  GL_ARG(a->kind != GL_APP_PAGERANK_VC, "an app on a vertex-cut fragment reports oids itself: no vertex map");
   if (vm) {
     gl_vm_view v;
     GL_TRY(gl_vm_view_get(vm, &v));
@@ -123,6 +125,9 @@ int gl_app_create(gl_app_t** out, int kind, gl_frag_t* frag, gl_comm_t* comm,
     case GL_APP_KCLIQUE: a = make_kclique(); break;
     case GL_APP_BC: a = make_bc(); break;
     case GL_APP_LCC_DIRECTED: a = make_lcc_directed(); break;
+    case GL_APP_PAGERANK_VC:
+      set_error("GL_APP_PAGERANK_VC runs on a vertex-cut fragment: use gl_vc_app_create");
+      return GL_ERR_ARG;
     default:
       set_error("unknown app kind %d", kind);
       return GL_ERR_ARG;
@@ -141,6 +146,32 @@ int gl_app_create(gl_app_t** out, int kind, gl_frag_t* frag, gl_comm_t* comm,
     set_error("fragment has fnum=%u: a communicator is required", frag->fnum);
     st = GL_ERR_COMM;
   }
+  if (st == GL_OK) st = a->Setup();
+  if (st != GL_OK) {
+    gl_app_destroy(a);
+    return st;
+  }
+  *out = a;
+  return GL_OK;
+}
+
+int gl_vc_app_create(gl_app_t** out, int kind, gl_vcfrag_t* frag, gl_comm_t* comm, const gl_app_config* cfg) {
+  GL_ARG(out && frag, "null argument");
+  if (kind != GL_APP_PAGERANK_VC) {
+    set_error("app kind %d does not run on a vertex-cut fragment (GL_APP_PAGERANK_VC only)", kind);
+    return GL_ERR_ARG;
+  }
+  gl_app* a = make_pagerank_vc(frag);
+  a->kind = kind;
+  a->comm = comm;
+  if (cfg) a->cfg = *cfg; else gl_app_config_default(&a->cfg);
+  memset(&a->fv, 0, sizeof(a->fv));
+  a->fv.fid = frag->fid;
+  a->fv.fnum = frag->fnum;
+  a->fv.fid_offset = 31;
+  a->fv.id_mask = 0x7fffffffu;
+  a->fv.total_vnum = frag->n;
+  int st = a->eng.init(nullptr);
   if (st == GL_OK) st = a->Setup();
   if (st != GL_OK) {
     gl_app_destroy(a);
@@ -227,8 +258,15 @@ int gl_app_result(gl_app_t* a, void* host_out, size_t bytes) {
 }
 
 int gl_app_result_oids(gl_app_t* a, int64_t* host_out, size_t count) {
-  GL_ARG(a && host_out && count >= a->frag->ivnum, "bad argument");
-  const gl_frag* f = a->frag;
+  GL_ARG(a && host_out, "null argument");
+  return a->ResultOids(host_out, count);
+}
+
+}  // extern "C"
+
+int gl_app::ResultOids(int64_t* host_out, size_t count) {
+  GL_ARG(count >= frag->ivnum, "bad argument");
+  const gl_frag* f = frag;
   if (!f->h_inner_oids.empty()) {
     memcpy(host_out, f->h_inner_oids.data(), sizeof(int64_t) * f->ivnum);
   } else {
@@ -236,6 +274,8 @@ int gl_app_result_oids(gl_app_t* a, int64_t* host_out, size_t count) {
   }
   return GL_OK;
 }
+
+extern "C" {
 
 void gl_app_destroy(gl_app_t* a) {
   if (!a) return;
