@@ -355,6 +355,29 @@ GL_DEV bool front_test(const PullArgs& a, const uint32_t* cur, uint32_t id) {
   return (cur[id >> 5] >> (id & 31)) & 1u;
 }
 
+// Stage-1 probes of one nibble of a candidate word: the candidates among its four vertices (bits of
+// `nib`) whose hub neighbour (h) is in the frontier.  Branch-free: every probe is an unconditional load
+// (index 0 / hub_dummy when the lane is not a candidate) so that the loads of a nibble are all in
+// flight together instead of forming a chain of dependent branches.
+template <bool kGlobal>
+GL_DEV uint32_t pull_probe_nibble(const PullArgs& a, const uint32_t* __restrict__ cur, uint32_t nib, uint4 h) {
+  const bool c0 = (nib & 1u) && h.x != kInfU32;
+  const bool c1 = (nib & 2u) && h.y != kInfU32;
+  const bool c2 = (nib & 4u) && h.z != kInfU32;
+  const bool c3 = (nib & 8u) && h.w != kInfU32;
+  const uint32_t dummy = kGlobal ? a.hub_dummy : 0u;
+  const uint32_t i0 = c0 ? h.x : dummy, i1 = c1 ? h.y : dummy;
+  const uint32_t i2 = c2 ? h.z : dummy, i3 = c3 ? h.w : dummy;
+  const bool t0 = front_test<kGlobal>(a, cur, i0), t1 = front_test<kGlobal>(a, cur, i1);
+  const bool t2 = front_test<kGlobal>(a, cur, i2), t3 = front_test<kGlobal>(a, cur, i3);
+  uint32_t r = 0;
+  r |= (c0 && t0) ? 1u : 0u;
+  r |= (c1 && t1) ? 2u : 0u;
+  r |= (c2 && t2) ? 4u : 0u;
+  r |= (c3 && t3) ? 8u : 0u;
+  return r;
+}
+
 // One super-tile = 8192 vertices = 256 words; thread t owns word t: it probes
 // the hub neighbour of each of its (up to 32) candidates with eight
 // independent 16-byte loads in flight (stage 1), hands the unresolved ones to
@@ -392,31 +415,38 @@ GL_DEV bool bfs_pull_phase(PullSmem& sm, const PullArgs& a,
     if (kTail && make_list) sm.cand[threadIdx.x] = word;
     // ---- stage 1 ----
     uint32_t res = 0;
-    if (word) {
+    if (kTail) {
+      // The hub neighbours of a warp's 32 words are 4 KB in a row.  Lane l reads 16 bytes of them per
+      // step, so that a warp load covers 4 lines: step j brings the 32 entries of lanes 4j..4j+3, and
+      // lane l probes nibble l % 8 of lane 4j + l / 8.  (A thread reading its own 128 bytes made every
+      // warp load touch 32 lines, eight times per line.)  The nibbles' results meet in the owning lane.
+      if (__any_sync(0xffffffffu, word != 0)) {
+        const uint32_t lane = lane_id();
+        const uint4* wp = (const uint4*) (a.hub_nbr + (vbase - lane * 32)) + lane;
+#pragma unroll 2
+        for (int j = 0; j < 8; ++j) {
+          const uint32_t nib = (__shfl_sync(0xffffffffu, word, 4 * j + (lane >> 3)) >> (4 * (lane & 7))) & 0xFu;
+          uint4 h = make_uint4(kInfU32, kInfU32, kInfU32, kInfU32);
+          if (nib) h = wp[32 * j];
+          uint32_t r = pull_probe_nibble<kGlobal>(a, cur, nib, h) << (4 * (lane & 7));
+          r |= __shfl_xor_sync(0xffffffffu, r, 1);
+          r |= __shfl_xor_sync(0xffffffffu, r, 2);
+          r |= __shfl_xor_sync(0xffffffffu, r, 4);
+          r = __shfl_sync(0xffffffffu, r, (lane & 3) * 8);
+          if ((lane >> 2) == (uint32_t) j) res = r;
+        }
+      }
+      scanned += __popc(word);
+    } else if (word) {
+      // (the stand-alone and several-fragment pulls keep the per-thread read: not measured with the
+      // warp-strided one, and the several-fragment kernels already spill at 64 registers)
       const uint4* hp = (const uint4*) (a.hub_nbr + vbase);
-      // branch-free: every probe is an unconditional load (index 0 when the
-      // lane is not a candidate) so that the loads of one iteration are all
-      // in flight together instead of forming a chain of dependent branches
 #pragma unroll 2
       for (int j = 0; j < 8; ++j) {
         const uint32_t nib = (word >> (4 * j)) & 0xFu;
         uint4 h = make_uint4(kInfU32, kInfU32, kInfU32, kInfU32);
         if (nib) h = hp[j];
-        const bool c0 = (nib & 1u) && h.x != kInfU32;
-        const bool c1 = (nib & 2u) && h.y != kInfU32;
-        const bool c2 = (nib & 4u) && h.z != kInfU32;
-        const bool c3 = (nib & 8u) && h.w != kInfU32;
-        const uint32_t dummy = kGlobal ? a.hub_dummy : 0u;
-        const uint32_t i0 = c0 ? h.x : dummy, i1 = c1 ? h.y : dummy;
-        const uint32_t i2 = c2 ? h.z : dummy, i3 = c3 ? h.w : dummy;
-        const bool t0 = front_test<kGlobal>(a, cur, i0), t1 = front_test<kGlobal>(a, cur, i1);
-        const bool t2 = front_test<kGlobal>(a, cur, i2), t3 = front_test<kGlobal>(a, cur, i3);
-        uint32_t r = 0;
-        r |= (c0 && t0) ? 1u : 0u;
-        r |= (c1 && t1) ? 2u : 0u;
-        r |= (c2 && t2) ? 4u : 0u;
-        r |= (c3 && t3) ? 8u : 0u;
-        res |= r << (4 * j);
+        res |= pull_probe_nibble<kGlobal>(a, cur, nib, h) << (4 * j);
       }
       scanned += __popc(word);
     }
