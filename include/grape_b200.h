@@ -415,9 +415,11 @@ typedef enum {
                           source_oid)  result: gl_bc_value, see below          */
   GL_APP_LCC_DIRECTED = 11,  /* lcc/lcc_directed.h (LCCDirected)  result: double,
                                 see below                                        */
-  GL_APP_PAGERANK_VC = 12   /* pagerank/pagerank_vc.h (PageRankVC, run_app --vc) on a
+  GL_APP_PAGERANK_VC = 12,  /* pagerank/pagerank_vc.h (PageRankVC, run_app --vc) on a
                                gl_vcfrag_t: created by gl_vc_app_create only;
                                result: double per master vertex, see below      */
+  GL_APP_CDLP_DIRECTED = 13 /* cuda/cdlp/cdlp.h on kBothOutIn (--directed)
+                               result: int64 label, see below                   */
 } gl_app_kind;
 
 /* ------------------------------------------------------------------ *
@@ -513,6 +515,26 @@ void gl_vcfrag_destroy(gl_vcfrag_t*);
  *     2^32 edges, can wrap on hubs.
  * Where every pair has fewer than 256 entries and the counts fit 32 bits, the result equals the
  * reference's bit for bit. */
+
+/* GL_APP_CDLP_DIRECTED: label propagation over the in- and out-neighbours of a directed graph (the
+ * reference's run_cuda_app --application cdlp --directed, the LDBC Graphalytics directed CDLP), one
+ * int64 label per inner vertex in lid order, as for GL_APP_CDLP: labels are kept as gids and mapped
+ * to oids on output, and gl_app_set_vertex_map works the same way.  It needs a directed fragment with
+ * its in-edges (gl_frag_desc.ie / kBothOutIn): an undirected fragment (use GL_APP_CDLP there) and a
+ * directed one without ie are refused at gl_app_create with GL_ERR_ARG.  Uses max_round only; every
+ * other gl_app_config field is ignored; edge data is ignored.
+ *   Labels start as the vertex's own id; each of max_round rounds updates all vertices at once.
+ *   The candidates of inner vertex v are the labels of ie(v) plus the labels of oe(v), with
+ *   multiplicity: a reciprocal pair u <-> v counts twice, a self loop twice (once in oe, once in ie),
+ *   every repeated edge once per copy.
+ *   The new label is the label with the highest count; ties go to the smallest label.
+ *   A vertex with |ie(v)| + |oe(v)| = 0 keeps its label; one with only in-edges updates (GL_APP_CDLP
+ *   keeps the label of a vertex without out-edges).  max_round = 0 returns the identity labelling.
+ * Ties are broken on the smallest gid, as GL_APP_CDLP does: under the segment partitioner that is the
+ * reference's smallest-oid rule; on hash or map partitions gid order is not oid order (see DESIGN.md).
+ * Directed CDLP on edge list E equals GL_APP_CDLP on the undirected fragment built from E, whose row
+ * of u is oe(u) + ie(u) as a multiset.  GL_APP_CDLP on a directed fragment is unchanged (out-edges
+ * only). */
 
 /* GL_APP_BC: single-source betweenness centrality, one gl_bc_value per inner vertex in lid order: the
  * reference's Output() line `oid c sigma depth` (gl_app_result_oids gives the oid).  A directed fragment
@@ -635,6 +657,8 @@ int gl_vc_app_create(gl_app_t** out, int kind, gl_vcfrag_t* frag, gl_comm_t* com
  *     1 runs in PEval).  Several fragments: the same with this fragment's ivnum and entries.  CDLP's
  *     step_entries is the size of the CSR its gather and sort are launched over, recorded by the host,
  *     not counted by a kernel.
+ *   CDLP_DIRECTED: as CDLP, with step_entries = the ie entries plus the oe entries of the fragment's
+ *     inner rows (both gathers and sorts); supersteps = max_round + 1, touched_vertices = ivnum x rounds.
  *   LCC, one fragment: step 1 counts the triangles: step_frontier = ivnum, step_entries = for every
  *     entry (v, u) of the degree-ordered DAG, the length of u's DAG row; supersteps = 3.
  *   LCC_DIRECTED: step 1 counts the triangles (mode 2): step_frontier = ivnum, step_entries = for every
