@@ -106,8 +106,11 @@ int build_hub_order(cudaStream_t s, const uint64_t* rp, uint32_t n, DevBuf<uint3
 int build_permuted_csr(cudaStream_t s, const uint64_t* rp, const uint32_t* col, uint64_t m, uint32_t n,
                        const uint32_t* order, const uint32_t* perm, DevBuf<uint64_t>* rp_out, DevBuf<uint32_t>* col_out,
                        const void* w4 = nullptr, DevBuf<uint32_t>* w4_out = nullptr, bool sort_rows = true);
-// every row [rp[i], rp[i+1]) of *col sorted ascending (the array is replaced by a sorted copy)
-int sort_csr_rows(cudaStream_t s, const uint64_t* rp, uint32_t n, uint64_t m, DevBuf<uint32_t>* col);
+// every row [rp[i], rp[i+1]) of *col sorted ascending, the entries of *val (when non-null) moved with their
+// keys (both arrays are replaced by sorted copies); V is uint32_t or uint64_t
+template <typename V = uint32_t>
+int sort_csr_rows(cudaStream_t s, const uint64_t* rp, uint32_t n, uint64_t m, DevBuf<uint32_t>* col,
+                  DevBuf<V>* val = nullptr);
 gl_app* make_bfs();
 gl_app* make_sssp_f32();
 gl_app* make_sssp_f64();

@@ -26,12 +26,9 @@
 //   4. fnum > 1: degrees of the outer copies come from the dense mirror sync; every fragment builds the
 //      rows of its inner vertices and replicates the peers' rows (PeerCsr); a fragment counts the
 //      cliques whose lowest vertex is one of its inner vertices; one peer all-reduce sums the counts.
-#include <cub/cub.cuh>
-
 #include <cstring>
-#include <vector>
 
-#include "apps_common.cuh"
+#include "dag_common.cuh"
 
 namespace gl {
 namespace {
@@ -88,62 +85,12 @@ GL_DEV bool contains(const uint32_t* a, uint32_t n, uint32_t x) {
 }
 
 // v -> u is kept when v ranks below u; a self loop and all but the first copy of a multi-edge are dropped
-GL_DEV bool kc_keep(const uint32_t* col, uint64_t b, uint64_t p, uint32_t v, uint32_t u, uint32_t dv, uint32_t du,
-                    uint32_t gv, uint32_t gu) {
-  return u != v && (p == b || col[p - 1] != u) && (dv < du || (dv == du && gv < gu));
-}
-
-__global__ void k_kc_count(const uint64_t* __restrict__ rp, const uint32_t* __restrict__ col,
-                           const uint32_t* __restrict__ deg, GidOf gid, uint32_t ivnum, uint64_t* cnt, KcCtl* ctl) {
-  const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
-  for (uint32_t v = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; v <= ivnum; v += warps) {
-    if (v == ivnum) {
-      if (lane_id() == 0) cnt[v] = 0;
-      continue;
-    }
-    const uint64_t b = rp[v], e = rp[v + 1];
-    const uint32_t dv = deg[v], gv = gid(v);
-    uint32_t k = 0;
-    for (uint64_t p = b + lane_id(); p < e; p += 32) {
-      const uint32_t u = col[p];
-      k += kc_keep(col, b, p, v, u, dv, deg[u], gv, gid(u));
-    }
-    k = warp_sum(k);
-    if (lane_id() == 0) {
-      cnt[v] = k;
-      if (k) atomicMax(&ctl->max_row, k);
-    }
+struct KcKeep {
+  GL_DEV bool operator()(const uint32_t* col, uint64_t b, uint64_t p, uint32_t v, uint32_t u, uint32_t dv,
+                         uint32_t du, uint32_t gv, uint32_t gu) const {
+    return u != v && (p == b || col[p - 1] != u) && (dv < du || (dv == du && gv < gu));
   }
-}
-
-// order-preserving fill: okey = gid of the head, osrc = lid of the tail
-__global__ void k_kc_fill(const uint64_t* __restrict__ rp, const uint32_t* __restrict__ col,
-                          const uint32_t* __restrict__ deg, GidOf gid, uint32_t ivnum,
-                          const uint64_t* __restrict__ orp, uint32_t* okey, uint32_t* osrc) {
-  const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
-  for (uint32_t v = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; v < ivnum; v += warps) {
-    const uint64_t b = rp[v], e = rp[v + 1];
-    const uint32_t dv = deg[v], gv = gid(v);
-    uint64_t o = orp[v];
-    for (uint64_t p0 = b; p0 < e; p0 += 32) {
-      const uint64_t p = p0 + lane_id();
-      bool k = false;
-      uint32_t gu = 0;
-      if (p < e) {
-        const uint32_t u = col[p];
-        gu = gid(u);
-        k = kc_keep(col, b, p, v, u, dv, deg[u], gv, gu);
-      }
-      const uint32_t mask = __ballot_sync(0xffffffffu, k);
-      if (k) {
-        const uint64_t at = o + __popc(mask & ((1u << lane_id()) - 1));
-        okey[at] = gu;
-        osrc[at] = v;
-      }
-      o += __popc(mask);
-    }
-  }
-}
+};
 
 struct KcArgs {
   Dag dag;
@@ -445,7 +392,7 @@ __global__ void __launch_bounds__(kTB, 1) k_kc_cta(KcArgs a, uint32_t n_b, uint3
 
 struct KCliqueApp : gl_app {
   int k = 0;
-  DevBuf<uint32_t> deg, okey, okey_tmp, osrc, queue, scratch;
+  DevBuf<uint32_t> deg, okey, osrc, queue, scratch;
   DevBuf<uint64_t> cnt, orp;
   DevBuf<KcCtl> d_ctl;
   PinnedBuf<KcCtl> h_ctl;
@@ -502,15 +449,10 @@ struct KCliqueApp : gl_app {
     const GidOf gid{fv.ivnum, fv.fid, fv.fid_offset, fv.ovgid};
     if (fv.ivnum) GL_LAUNCH(k_row_length<uint32_t>, (fv.ivnum + 255) / 256, 256, s, fv.oe_rp, fv.ivnum, deg.get());
     if (fv.fnum > 1) GL_TRY(mm.SyncValuesToGhosts(s, deg, 4));
-    GL_LAUNCH(k_kc_count, eng.sm_count * 8, 256, s, fv.oe_rp, fv.oe_col, deg, gid, fv.ivnum, cnt, d_ctl);
-    size_t tb = 0;
-    GL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt.get(), orp.get(), (int) (fv.ivnum + 1), s));
-    DevBuf<char> tmp;
-    GL_CUDA(tmp.alloc(std::max<size_t>(tb, 16)));
-    GL_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, cnt.get(), orp.get(), (int) (fv.ivnum + 1), s));
+    GL_LAUNCH(k_dag_count<KcKeep>, eng.sm_count * 8, 256, s, fv.oe_rp, fv.oe_col, deg, gid, fv.ivnum, KcKeep{}, cnt,
+              &d_ctl.get()->max_row);
     uint64_t total = 0;
-    GL_CUDA(cudaMemcpyAsync(&total, orp + fv.ivnum, 8, cudaMemcpyDeviceToHost, s));
-    GL_CUDA(cudaStreamSynchronize(s));
+    GL_TRY(dag_scan(s, cnt, orp, fv.ivnum, &total));
     // every rank takes the same decision, so no rank is left waiting in the next collective
     long long most = (long long) total, unused = 0;
     double unused_d = 0;
@@ -530,23 +472,10 @@ struct KCliqueApp : gl_app {
       GL_CUDA(queue.alloc(std::max<uint64_t>(om, 4)));
     }
     if (fv.ivnum && om) {
-      if (fv.fnum == 1) {
-        // gid == lid: rows come out sorted
-        GL_LAUNCH(k_kc_fill, eng.sm_count * 8, 256, s, fv.oe_rp, fv.oe_col, deg, gid, fv.ivnum, orp, okey, osrc);
-      } else {
-        // outer gids do not follow lid order
-        DevBuf<uint32_t> key_u;
-        GL_CUDA(key_u.alloc(om));
-        GL_LAUNCH(k_kc_fill, eng.sm_count * 8, 256, s, fv.oe_rp, fv.oe_col, deg, gid, fv.ivnum, orp, key_u, osrc);
-        size_t sb = 0;
-        GL_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, sb, key_u.get(), okey.get(), (int64_t) om,
-                                                   (int64_t) fv.ivnum, orp.get(), orp + 1, s));
-        DevBuf<char> st;
-        GL_CUDA(st.alloc(std::max<size_t>(sb, 16)));
-        GL_CUDA(cub::DeviceSegmentedSort::SortKeys(st, sb, key_u.get(), okey.get(), (int64_t) om,
-                                                   (int64_t) fv.ivnum, orp.get(), orp + 1, s));
-        GL_CUDA(cudaStreamSynchronize(s));
-      }
+      GL_LAUNCH(k_dag_fill<KcKeep>, eng.sm_count * 8, 256, s, fv.oe_rp, fv.oe_col, deg, gid, fv.ivnum, KcKeep{}, orp,
+                okey, nullptr, osrc);
+      // several fragments: outer gids do not follow lid order
+      if (fv.fnum > 1) GL_TRY(sort_csr_rows(s, orp, fv.ivnum, om, &okey));
     }
     return dag.replicate(mm, s, fv, orp, okey, om);
   }

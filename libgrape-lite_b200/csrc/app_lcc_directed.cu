@@ -21,15 +21,11 @@
 //      by a warp, longer ones (R-MAT in-rows of hubs) by a CTA;
 //   3. several fragments: rows hold gids, sorted by gid (outer gids do not follow lid order), and every
 //      fragment replicates its peers' rows and weights (PeerCsr).
-// IncEval stage 0: one warp per oriented edge (v,u) intersects N+(u) with the sorted N+(v); for every
-// common x: tri[x] += w(v,u), tri[u] += w(v,x), tri[v] += w(u,x), in 64-bit atomics.  A triangle is
-// counted once, by the owner of its highest-ranked vertex; counts that land on outer copies go to their
-// owners as (lid, count) items, added in stage 1.
-#include <cub/cub.cuh>
-
-#include <vector>
-
-#include "apps_common.cuh"
+// IncEval (TriangleApp in dag_common.cuh, shared with app_lcc.cu) stage 0: one warp per oriented edge
+// (v,u) intersects N+(u) with the sorted N+(v); for every common x: tri[x] += w(v,u), tri[u] += w(v,x),
+// tri[v] += w(u,x), in 64-bit atomics.  A triangle is counted once, by the owner of its highest-ranked
+// vertex; counts that land on outer copies go to their owners as (lid, count) items, added in stage 1.
+#include "dag_common.cuh"
 
 namespace gl {
 namespace {
@@ -250,89 +246,14 @@ __global__ void k_lccd_split(const uint64_t* __restrict__ val, uint64_t om, uint
   }
 }
 
-// one warp per oriented edge (v,u); N+(u) and its weights come from the owner's replica
-__global__ void __launch_bounds__(256)
-k_lccd_tri(const uint64_t* __restrict__ orp, const uint32_t* __restrict__ okey, const uint32_t* __restrict__ olid,
-           const uint32_t* __restrict__ ow, const uint32_t* __restrict__ osrc, uint64_t om,
-           const uint64_t* const* __restrict__ t_orp, const uint32_t* const* __restrict__ t_key,
-           const uint32_t* const* __restrict__ t_w, int fid_offset, uint32_t id_mask,
-           unsigned long long* tri, ScanCtrl* ctrl) {
-  const uint64_t warps = ((uint64_t) gridDim.x * blockDim.x) >> 5;
-  uint64_t scanned = 0;
-  for (uint64_t ei = ((uint64_t) blockIdx.x * blockDim.x + threadIdx.x) >> 5; ei < om; ei += warps) {
-    const uint32_t v = osrc[ei], ug = okey[ei], ul = olid[ei];
-    const unsigned long long wvu = ow[ei];
-    const uint64_t vb = orp[v], ve = orp[v + 1];
-    const uint32_t g = ug >> fid_offset, l = ug & id_mask;
-    const uint64_t* rorp = t_orp[g];
-    const uint32_t* rkey = t_key[g];
-    const uint32_t* rw = t_w[g];
-    const uint64_t ub = rorp[l], ue = rorp[l + 1];
-    unsigned long long to_u = 0, to_v = 0;
-    for (uint64_t p = ub + lane_id(); p < ue; p += 32) {
-      const uint32_t x = rkey[p];
-      uint64_t lo = vb, hi = ve;
-      while (lo < hi) {
-        const uint64_t mid = (lo + hi) >> 1;
-        if (okey[mid] < x) lo = mid + 1; else hi = mid;
-      }
-      if (lo < ve && okey[lo] == x) {
-        atomicAdd(tri + olid[lo], wvu);
-        to_u += ow[lo];
-        to_v += rw[p];
-      }
-    }
-    to_u = warp_sum(to_u);
-    to_v = warp_sum(to_v);
-    if (lane_id() == 0) {
-      if (to_u) atomicAdd(tri + ul, to_u);
-      if (to_v) atomicAdd(tri + v, to_v);
-      scanned += ue - ub;
-    }
-  }
-  if (lane_id() == 0 && scanned) atomicAdd(&ctrl->scanned, (unsigned long long) scanned);
-}
-
 __global__ void k_lccd_orient_src(const uint64_t* __restrict__ orp, uint32_t ivnum, uint32_t* osrc) {
   const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
   for (uint32_t v = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; v < ivnum; v += warps)
     for (uint64_t p = orp[v] + lane_id(); p < orp[v + 1]; p += 32) osrc[p] = v;
 }
 
-__global__ void k_lccd_mark_remote(const unsigned long long* tri, uint32_t ivnum, uint32_t ovnum, uint32_t* remote) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < ovnum && tri[ivnum + i]) bit_set_atomic(remote, ivnum + i);
-}
-struct LccdPayload {
-  const unsigned long long* tri;
-  GL_DEV ItemU32I64 operator()(uint32_t v, uint32_t lid) const { return ItemU32I64{lid, 0u, (int64_t) tri[v]}; }
-};
-struct LccdApply {
-  unsigned long long* tri;
-  GL_DEV void operator()(const ItemU32I64& it, ScanAcc&) const {
-    atomicAdd(tri + it.lid, (unsigned long long) it.val);
-  }
-};
-
-__global__ void k_lccd_out(const uint32_t* dd, const unsigned long long* tri, uint32_t ivnum, double* out) {
-  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= ivnum) return;
-  const int64_t d = dd[v];
-  out[v] = d < 2 ? 0.0 : (double) tri[v] / (double) (d * (d - 1));
-}
-
-struct LccDirectedApp : gl_app {
-  DevBuf<uint64_t> cnt, orp;
-  DevBuf<uint32_t> deg, dd, okey, olid, ow, osrc, remote;
-  DevBuf<unsigned long long> tri;
-  DevBuf<double> out64;
-  uint64_t om = 0;
-  int stage = 0;
-  uint32_t tvnum = 0;
-  size_t words = 0;
-  PeerCsr peers;   // every fragment's oriented rows and weights (one fragment: its own)
-
-  size_t ResultElemBytes() const override { return sizeof(double); }
+struct LccDirectedApp : TriangleApp<true> {
+  DevBuf<uint32_t> dd;   // [ivnum] deduplicated degree
 
   int Setup() override {
     // the reference runs LCCDirected on kBothOutIn directed fragments only
@@ -345,27 +266,8 @@ struct LccDirectedApp : gl_app {
       set_error("lcc_directed needs the incoming adjacency (gl_frag_desc.ie / kBothOutIn)");
       return GL_ERR_ARG;
     }
-    tvnum = fv.ivnum + fv.ovnum;
-    words = bm_words(tvnum) + 1;
-    GL_CUDA(cnt.alloc((size_t) fv.ivnum + 1));
-    GL_CUDA(orp.alloc((size_t) fv.ivnum + 1));
-    GL_CUDA(deg.alloc(std::max<uint32_t>(tvnum, 1)));
     GL_CUDA(dd.alloc(std::max<uint32_t>(fv.ivnum, 1)));
-    GL_CUDA(tri.alloc(std::max<uint32_t>(tvnum, 1)));
-    GL_CUDA(out64.alloc(std::max<uint32_t>(fv.ivnum, 1)));
-    GL_TRY(mm.Init(comm, fv, sizeof(ItemU32I64)));
-    if (fv.fnum > 1) {
-      GL_CUDA(remote.alloc(words));
-      GL_TRY(mm.BuildMirrorPlan(eng.stream, fv));
-    }
-    return GL_OK;
-  }
-
-  int Init() override {
-    stage = 0;
-    GL_CUDA(cudaMemsetAsync(tri, 0, sizeof(unsigned long long) * std::max<uint32_t>(tvnum, 1), eng.stream));
-    if (remote) GL_CUDA(cudaMemsetAsync(remote, 0, sizeof(uint32_t) * words, eng.stream));
-    return GL_OK;
+    return TriangleApp::Setup();
   }
 
   // PEval: degrees, then the oriented rows with their weights (lcc_directed.h:146-240)
@@ -380,51 +282,23 @@ struct LccDirectedApp : gl_app {
       GL_LAUNCH(k_lccd_rows_warp<false>, eng.sm_count * 8, kTB, s, a);
       GL_LAUNCH(k_lccd_rows_cta<false>, eng.sm_count * 4, kTB, s, a);
     }
-    size_t tb = 0;
-    GL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt.get(), orp.get(), (int) (fv.ivnum + 1), s));
-    DevBuf<char> tmp;
-    GL_CUDA(tmp.alloc(std::max<size_t>(tb, 16)));
-    GL_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, cnt.get(), orp.get(), (int) (fv.ivnum + 1), s));
-    uint64_t total = 0;
-    GL_CUDA(cudaMemcpyAsync(&total, orp + fv.ivnum, 8, cudaMemcpyDeviceToHost, s));
-    GL_CUDA(cudaStreamSynchronize(s));
-    if (total != om || !okey) {
-      okey.reset();
-      olid.reset();
-      ow.reset();
-      osrc.reset();
-      om = total;
-      GL_CUDA(okey.alloc(std::max<uint64_t>(om, 4)));
-      GL_CUDA(ow.alloc(std::max<uint64_t>(om, 4)));
-      GL_CUDA(osrc.alloc(std::max<uint64_t>(om, 4)));
-      if (fv.fnum > 1) GL_CUDA(olid.alloc(std::max<uint64_t>(om, 4)));
-    }
+    GL_TRY(scan_and_resize());
     if (fv.ivnum && om) {
+      a.okey = okey;
       if (fv.fnum == 1) {
         // gid == lid: rows come out sorted, and okey doubles as the lid array
-        a.okey = okey;
         a.ow = ow;
         GL_LAUNCH(k_lccd_rows_warp<true>, eng.sm_count * 8, kTB, s, a);
         GL_LAUNCH(k_lccd_rows_cta<true>, eng.sm_count * 4, kTB, s, a);
       } else {
         // outer gids do not follow lid order: sort every row by gid, carrying (weight, lid)
-        DevBuf<uint32_t> key_u;
-        DevBuf<uint64_t> val_u, val_s;
-        GL_CUDA(key_u.alloc(om));
-        GL_CUDA(val_u.alloc(om));
-        GL_CUDA(val_s.alloc(om));
-        a.okey = key_u;
-        a.oval = val_u;
+        DevBuf<uint64_t> val;
+        GL_CUDA(val.alloc(om));
+        a.oval = val;
         GL_LAUNCH(k_lccd_rows_warp<true>, eng.sm_count * 8, kTB, s, a);
         GL_LAUNCH(k_lccd_rows_cta<true>, eng.sm_count * 4, kTB, s, a);
-        size_t sb = 0;
-        GL_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, sb, key_u.get(), okey.get(), val_u.get(), val_s.get(),
-                                                    (int64_t) om, (int64_t) fv.ivnum, orp.get(), orp + 1, s));
-        DevBuf<char> st;
-        GL_CUDA(st.alloc(std::max<size_t>(sb, 16)));
-        GL_CUDA(cub::DeviceSegmentedSort::SortPairs(st, sb, key_u.get(), okey.get(), val_u.get(), val_s.get(),
-                                                    (int64_t) om, (int64_t) fv.ivnum, orp.get(), orp + 1, s));
-        GL_LAUNCH(k_lccd_split, eng.sm_count * 8, 256, s, val_s, om, olid, ow);
+        GL_TRY(sort_csr_rows(s, orp, fv.ivnum, om, &okey, &val));
+        GL_LAUNCH(k_lccd_split, eng.sm_count * 8, 256, s, val, om, olid, ow);
       }
       GL_LAUNCH(k_lccd_orient_src, eng.sm_count * 8, 256, s, orp, fv.ivnum, osrc);
       GL_CUDA(cudaStreamSynchronize(s));
@@ -434,43 +308,7 @@ struct LccDirectedApp : gl_app {
     return GL_OK;
   }
 
-  // IncEval: weighted triangle counting (stage 1, lcc_directed.h:241-350), then the counts of outer
-  // copies are added at their owners (stage 2, :351-357)
-  int IncEval() override {
-    cudaStream_t s = eng.stream;
-    if (stage == 0) {
-      stage = 1;
-      GL_TRY(eng.reset_ctrl());
-      if (om)
-        GL_LAUNCH(k_lccd_tri, eng.sm_count * 8, 256, s, orp, okey, fv.fnum > 1 ? olid.get() : okey.get(), ow, osrc,
-                  om, peers.d_rp, peers.d_col, peers.d_w, fv.fid_offset, fv.id_mask, tri, eng.ctrl);
-      if (fv.fnum > 1) {
-        if (fv.ovnum) GL_LAUNCH(k_lccd_mark_remote, (fv.ovnum + 255) / 256, 256, s, tri, fv.ivnum, fv.ovnum, remote);
-        MsgView mv = mm.view();
-        GL_LAUNCH((k_pack_outer<ItemU32I64, LccdPayload>), eng.sm_count * 4, kTB, s, remote, fv.ivnum, fv.ovnum,
-                  fv.ovgid, mv, LccdPayload{tri}, 0, nullptr);
-      }
-      GL_TRY(eng.fetch_ctrl());
-      note_step(eng.h_ctrl->scanned, fv.ivnum, 2);
-      q_touched += fv.ivnum;
-      mm.ForceContinue();
-    } else {
-      if (stage == 1 && fv.fnum > 1) {
-        MsgView mv = mm.view();
-        GL_LAUNCH((k_unpack<ItemU32I64, LccdApply>), eng.sm_count * 4, kTB, s, mv, LccdApply{tri}, eng.ctrl);
-      }
-      stage = 2;
-    }
-    return GL_OK;
-  }
-
-  int Result(void* host_out, size_t) override {
-    if (fv.ivnum == 0) return GL_OK;
-    GL_LAUNCH(k_lccd_out, (fv.ivnum + 255) / 256, 256, eng.stream, dd, tri, fv.ivnum, out64);
-    GL_CUDA(cudaMemcpyAsync(host_out, out64, sizeof(double) * fv.ivnum, cudaMemcpyDeviceToHost, eng.stream));
-    GL_CUDA(cudaStreamSynchronize(eng.stream));
-    return GL_OK;
-  }
+  int Result(void* host_out, size_t) override { return WriteResult(host_out, dd, 1.0); }
 };
 
 }  // namespace

@@ -97,28 +97,7 @@ int build_permuted_csr(cudaStream_t s, const uint64_t* rp, const uint32_t* col, 
   // rows sorted by the new ids = by descending degree of the neighbour: the
   // most promising parents come first in a pull scan, and the entries of a
   // row that fall into the same bitmap word are adjacent
-  if (n && m && sort_rows) {
-    DevBuf<uint32_t> sorted;
-    GL_CUDA(sorted.alloc(m + 16));
-    size_t sb = 0;
-    DevBuf<char> st;
-    if (!w_p) {
-      GL_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, sb, col_p.get(), sorted.get(), (int64_t) m, (int64_t) n, rp_p.get(), rp_p + 1, s));
-      GL_CUDA(st.alloc(std::max<size_t>(sb, 16)));
-      GL_CUDA(cub::DeviceSegmentedSort::SortKeys(st, sb, col_p.get(), sorted.get(), (int64_t) m, (int64_t) n, rp_p.get(), rp_p + 1, s));
-    } else {
-      DevBuf<uint32_t> w_sorted;
-      GL_CUDA(w_sorted.alloc(m + 16));
-      GL_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, sb, col_p.get(), sorted.get(), w_p.get(), w_sorted.get(), (int64_t) m, (int64_t) n, rp_p.get(), rp_p + 1, s));
-      GL_CUDA(st.alloc(std::max<size_t>(sb, 16)));
-      GL_CUDA(cub::DeviceSegmentedSort::SortPairs(st, sb, col_p.get(), sorted.get(), w_p.get(), w_sorted.get(), (int64_t) m, (int64_t) n, rp_p.get(), rp_p + 1, s));
-      GL_CUDA(cudaStreamSynchronize(s));
-      w_p = std::move(w_sorted);
-    }
-    GL_CUDA(cudaStreamSynchronize(s));
-    st.reset();
-    col_p = std::move(sorted);
-  }
+  if (sort_rows) GL_TRY(sort_csr_rows(s, rp_p, n, m, &col_p, w4 ? &w_p : nullptr));
   GL_CUDA(cudaStreamSynchronize(s));
   deg.reset();
   tmp.reset();
@@ -128,19 +107,33 @@ int build_permuted_csr(cudaStream_t s, const uint64_t* rp, const uint32_t* col, 
   return GL_OK;
 }
 
-int sort_csr_rows(cudaStream_t s, const uint64_t* rp, uint32_t n, uint64_t m, DevBuf<uint32_t>* col) {
+template <typename V>
+int sort_csr_rows(cudaStream_t s, const uint64_t* rp, uint32_t n, uint64_t m, DevBuf<uint32_t>* col, DevBuf<V>* val) {
   if (!n || !m) return GL_OK;
   DevBuf<uint32_t> sorted;
+  DevBuf<V> val_sorted;
   GL_CUDA(sorted.alloc(m + 16));
+  if (val) GL_CUDA(val_sorted.alloc(m + 16));
   size_t sb = 0;
   DevBuf<char> st;
-  GL_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, sb, col->get(), sorted.get(), (int64_t) m, (int64_t) n, rp, rp + 1, s));
-  GL_CUDA(st.alloc(std::max<size_t>(sb, 16)));
-  GL_CUDA(cub::DeviceSegmentedSort::SortKeys(st, sb, col->get(), sorted.get(), (int64_t) m, (int64_t) n, rp, rp + 1, s));
+  if (val) {
+    GL_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, sb, col->get(), sorted.get(), val->get(), val_sorted.get(),
+                                                (int64_t) m, (int64_t) n, rp, rp + 1, s));
+    GL_CUDA(st.alloc(std::max<size_t>(sb, 16)));
+    GL_CUDA(cub::DeviceSegmentedSort::SortPairs(st, sb, col->get(), sorted.get(), val->get(), val_sorted.get(),
+                                                (int64_t) m, (int64_t) n, rp, rp + 1, s));
+  } else {
+    GL_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, sb, col->get(), sorted.get(), (int64_t) m, (int64_t) n, rp, rp + 1, s));
+    GL_CUDA(st.alloc(std::max<size_t>(sb, 16)));
+    GL_CUDA(cub::DeviceSegmentedSort::SortKeys(st, sb, col->get(), sorted.get(), (int64_t) m, (int64_t) n, rp, rp + 1, s));
+  }
   GL_CUDA(cudaStreamSynchronize(s));
   st.reset();
   *col = std::move(sorted);
+  if (val) *val = std::move(val_sorted);
   return GL_OK;
 }
+template int sort_csr_rows(cudaStream_t, const uint64_t*, uint32_t, uint64_t, DevBuf<uint32_t>*, DevBuf<uint32_t>*);
+template int sort_csr_rows(cudaStream_t, const uint64_t*, uint32_t, uint64_t, DevBuf<uint32_t>*, DevBuf<uint64_t>*);
 
 }  // namespace gl
