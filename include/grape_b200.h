@@ -399,7 +399,10 @@ typedef enum {
   GL_APP_BFS = 0,      /* cuda/bfs/bfs.h        result: int64 depth            */
   GL_APP_SSSP = 1,     /* cuda/sssp/sssp.h      result: double (f32/f64 math)  */
   GL_APP_WCC = 2,      /* cuda/wcc/wcc.h        result: int64 oid of min-gid   */
-  GL_APP_PAGERANK = 3, /* cuda/pagerank/pagerank.h result: double              */
+  GL_APP_PAGERANK = 3, /* cuda/pagerank/pagerank.h result: double; on a directed
+                          fragment it follows pagerank_parallel.h (a vertex without
+                          out-edges keeps base each round); the Graphalytics
+                          directed PageRank is GL_APP_PAGERANK_DIRECTED         */
   GL_APP_CDLP = 4,     /* cuda/cdlp/cdlp.h      result: int64 label            */
   GL_APP_LCC = 5,      /* cuda/lcc/lcc_opt.h    result: double                 */
   GL_APP_WCC_OPT = 6,  /* cuda/wcc/wcc_opt.h (union-find) result: as GL_APP_WCC  */
@@ -418,8 +421,11 @@ typedef enum {
   GL_APP_PAGERANK_VC = 12,  /* pagerank/pagerank_vc.h (PageRankVC, run_app --vc) on a
                                gl_vcfrag_t: created by gl_vc_app_create only;
                                result: double per master vertex, see below      */
-  GL_APP_CDLP_DIRECTED = 13 /* cuda/cdlp/cdlp.h on kBothOutIn (--directed)
+  GL_APP_CDLP_DIRECTED = 13, /* cuda/cdlp/cdlp.h on kBothOutIn (--directed)
                                result: int64 label, see below                   */
+  GL_APP_PAGERANK_DIRECTED = 14 /* pagerank/pagerank_directed.h (PageRankDirected,
+                                   run_app_opt --application pagerank --directed)
+                                   result: double, see below                    */
 } gl_app_kind;
 
 /* ------------------------------------------------------------------ *
@@ -535,6 +541,37 @@ void gl_vcfrag_destroy(gl_vcfrag_t*);
  * Directed CDLP on edge list E equals GL_APP_CDLP on the undirected fragment built from E, whose row
  * of u is oe(u) + ie(u) as a multiset.  GL_APP_CDLP on a directed fragment is unchanged (out-edges
  * only). */
+
+/* GL_APP_PAGERANK_DIRECTED: the directed PageRank of LDBC Graphalytics (the reference's PageRankDirected,
+ * run_app_opt --application pagerank --directed), one double per inner vertex in lid order.  It needs a
+ * directed fragment with its in-edges (gl_frag_desc.ie / kBothOutIn): an undirected fragment (use
+ * GL_APP_PAGERANK there) and a directed one without ie are refused at gl_app_create with GL_ERR_ARG.
+ * Uses pr_delta (d) and max_round (R); every other gl_app_config field, pr_pull included, is ignored;
+ * edge data is ignored.  N = vertices of the whole group; deg(v) = the entries of v's out-row
+ * (duplicates count, a self loop counts once); v is dangling when deg(v) = 0; D = the dangling vertices
+ * of the group.
+ *   R <= 0: nothing runs; every result is 0.0 (the reference's zero-initialised result); supersteps = 1.
+ *   PEval: p = 1/N; x[v] = p / deg(v), or p when v is dangling; S = p * D.
+ *   Round k = 1..R: base = (1 - d)/N + d * S/N;
+ *          c(v) = d * (sum of x[w] over the entries w of ie(v)) + base;
+ *          x[v] = c(v) when v is dangling, else c(v) / deg(v);
+ *          k < R: S = the sum of c(v) over the dangling vertices of the group.
+ *   Output: x[v] * deg(v) for a non-dangling v (the reference's multiply-back, (c / deg) * deg, not c);
+ *          x[v] for a dangling v.
+ * A vertex without out-edges keeps what arrives over its in-edges, and the mass the dangling vertices
+ * hold is spread evenly over every vertex in the next round, so for R >= 1 the results of the group
+ * sum to 1 up to rounding.  GL_APP_PAGERANK on a directed fragment does not have this property: it
+ * resets such a vertex to base every round.
+ * Everything is f64, and every sum has a fixed order: an in-row in the row tiers of GL_APP_PAGERANK_VC
+ * (a thread up to 32 entries, a warp up to 4096, longer rows in 4096-entry chunks folded in order), S
+ * from per-CTA partials folded in CTA order and, on several fragments, in fid order.  The same input
+ * on the same fragments gives bit-identical output on every run.
+ * Stats: supersteps = R + 1; step k = round k (1..R), mode 2, step_frontier = ivnum, step_entries = the
+ *   fragment's ie entries (a host count); touched_vertices = ivnum x R.  msg_bytes_sent (F > 1) =
+ *   R x 8 M + (R - 1) x 8 (F - 1), where M = the outer copies of this fragment's inner vertices held
+ *   by the other fragments (the dense mirror sync of x after PEval and after rounds 1..R-1) and 8 (F - 1)
+ *   is the value S this fragment sends to its peers in each all-reduce after rounds 1..R-1.
+ *   R <= 0: 0. */
 
 /* GL_APP_BC: single-source betweenness centrality, one gl_bc_value per inner vertex in lid order: the
  * reference's Output() line `oid c sigma depth` (gl_app_result_oids gives the oid).  A directed fragment
@@ -659,6 +696,7 @@ int gl_vc_app_create(gl_app_t** out, int kind, gl_vcfrag_t* frag, gl_comm_t* com
  *     not counted by a kernel.
  *   CDLP_DIRECTED: as CDLP, with step_entries = the ie entries plus the oe entries of the fragment's
  *     inner rows (both gathers and sorts); supersteps = max_round + 1, touched_vertices = ivnum x rounds.
+ *   PAGERANK_DIRECTED: see GL_APP_PAGERANK_DIRECTED above.
  *   LCC, one fragment: step 1 counts the triangles: step_frontier = ivnum, step_entries = for every
  *     entry (v, u) of the degree-ordered DAG, the length of u's DAG row; supersteps = 3.
  *   LCC_DIRECTED: step 1 counts the triangles (mode 2): step_frontier = ivnum, step_entries = for every

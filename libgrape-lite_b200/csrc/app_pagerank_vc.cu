@@ -7,11 +7,8 @@
 // into the new rank / degree and SCATTERED back to every fragment holding the vertex.
 //
 // Every sum has one fixed order, so the output is bit-identical from run to run (the reference adds
-// with f64 atomics in thread order).  That rules out the atomic row flushes of k_dense_pull, whose
-// partial sums of a row that spans several warps or tiles land in scheduling order: a row is owned
-// by one thread (up to kVcShort entries, in sequence), one warp (up to kVcChunk entries, lane stride
-// 32 then a shuffle tree), or split into kVcChunk-entry chunks whose warp sums are folded in chunk
-// order by a second kernel.
+// with f64 atomics in thread order): the row tiers of row_tiers.cuh (a thread, a warp, or chunks
+// folded in chunk order by a second kernel).
 //
 // Gather / scatter (F > 1) are dense peer stores into the communicator's mirror slots: a fragment
 // stores the partial-sum slice of every other fragment's master range it holds into that owner's
@@ -23,14 +20,11 @@
 // every fragment has passed the scatter barrier, i.e. after every fold has read its slices.
 #include <cmath>
 
-#include "apps_common.cuh"
+#include "row_tiers.cuh"
 #include "vcfrag.h"
 
 namespace gl {
 namespace {
-
-constexpr uint32_t kVcShort = 32;     // rows up to this length: one thread, sequential sum
-constexpr uint32_t kVcChunk = 4096;   // rows up to this length: one warp; longer: chunks of this many entries
 
 struct VcSlice {
   double* ptr;     // peer slot (put) or my slot (copy-in)
@@ -38,55 +32,28 @@ struct VcSlice {
   uint64_t cnt;
 };
 
+struct VcStore {
+  double* next;
+  GL_DEV void operator()(uint32_t r, double s) const { next[r] = s; }
+};
+
 __global__ void __launch_bounds__(kTB)
 k_vc_pull(const uint64_t* __restrict__ rp, const uint32_t* __restrict__ col, uint32_t nl,
           const double* __restrict__ curr, double* __restrict__ next) {
-  const uint32_t lane = lane_id();
-  const uint64_t nwarps = (uint64_t) gridDim.x * (kTB / 32);
-  for (uint64_t g = ((uint64_t) blockIdx.x * kTB + threadIdx.x) / 32; g * 32 < nl; g += nwarps) {
-    const uint64_t r = g * 32 + lane;
-    const bool ok = r < nl;
-    const uint64_t b = ok ? rp[r] : 0, e = ok ? rp[r + 1] : 0;
-    const uint64_t deg = e - b;
-    double s = 0.0;
-    if (deg <= kVcShort)
-      for (uint64_t p = b; p < e; ++p) s += curr[col[p]];
-    uint32_t med = __ballot_sync(0xffffffffu, ok && deg > kVcShort && deg <= kVcChunk);
-    while (med) {
-      const int j = __ffs(med) - 1;
-      med &= med - 1;
-      const uint64_t rb = __shfl_sync(0xffffffffu, b, j), re = __shfl_sync(0xffffffffu, e, j);
-      double t = 0.0;
-      for (uint64_t p = rb + lane; p < re; p += 32) t += curr[col[p]];
-      t = warp_sum(t);
-      if ((int) lane == j) s = t;
-    }
-    if (ok && deg <= kVcChunk) next[r] = s;
-  }
+  VcStore out{next};
+  tier_rows(rp, col, nl, curr, out);
 }
 
-// one warp per kVcChunk-entry chunk [cb[i], ce[i]) of a long row
 __global__ void __launch_bounds__(kTB)
 k_vc_chunks(const uint64_t* __restrict__ cb, const uint64_t* __restrict__ ce, uint32_t nitems,
             const uint32_t* __restrict__ col, const double* __restrict__ curr, double* __restrict__ csum) {
-  const uint32_t lane = lane_id();
-  const uint32_t nwarps = gridDim.x * (kTB / 32);
-  for (uint32_t i = (blockIdx.x * kTB + threadIdx.x) / 32; i < nitems; i += nwarps) {
-    double t = 0.0;
-    for (uint64_t p = cb[i] + lane; p < ce[i]; p += 32) t += curr[col[p]];
-    t = warp_sum(t);
-    if (lane == 0) csum[i] = t;
-  }
+  tier_chunks(cb, ce, nitems, col, curr, csum);
 }
 
-// next[long row j] = its chunk sums [off[j], off[j+1]) in chunk order
 __global__ void k_vc_long(const uint32_t* __restrict__ rows, const uint32_t* __restrict__ off, uint32_t nlong,
                           const double* __restrict__ csum, double* __restrict__ next) {
-  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= nlong) return;
-  double s = 0.0;
-  for (uint32_t i = off[j]; i < off[j + 1]; ++i) s += csum[i];
-  next[rows[j]] = s;
+  VcStore out{next};
+  tier_long(rows, off, nlong, csum, out);
 }
 
 // dense slices of `src` into peer slots (blockIdx.y = slice)
@@ -153,12 +120,9 @@ struct PageRankVcApp : gl_app {
   gl_vcfrag* vf = nullptr;
   uint32_t nl = 0;
   uint64_t nm = 0, mlid = 0;   // own masters and the local id of the first
-  DevBuf<double> curr, next, deg, res, csum;
+  DevBuf<double> curr, next, deg, res;
   DevBuf<unsigned long long> d_ndangling;
-  // long rows: chunk items [cb, ce) and, per long row, its item range
-  DevBuf<uint64_t> cb, ce;
-  DevBuf<uint32_t> lrows, loff;
-  uint32_t nitems = 0, nlong = 0;
+  TierLongRows lr;   // rows longer than kTierChunk entries
   // gather / scatter tables (F > 1)
   DevBuf<VcSlice> d_put, d_copy;
   uint32_t nput = 0, ncopy = 0;
@@ -192,7 +156,7 @@ struct PageRankVcApp : gl_app {
     GL_CUDA(deg.alloc(std::max<uint64_t>(nm, 1)));
     GL_CUDA(res.alloc(std::max<uint64_t>(nm, 1)));
     GL_CUDA(d_ndangling.alloc(1));
-    GL_TRY(plan_long_rows());
+    GL_TRY(lr.plan(vf->rp, nl));
     if (vf->fnum > 1) {
       const uint64_t need = 8 * vf->mvc;
       if (!comm || !comm->opened || comm->fnum != vf->fnum || comm->fid != vf->fid) {
@@ -206,36 +170,6 @@ struct PageRankVcApp : gl_app {
     }
     GL_TRY(mm.Init(comm, fv, 8));
     return plan_gather_scatter();
-  }
-
-  // Rows longer than kVcChunk entries: their chunk items, from the row pointers (host copy, once).
-  int plan_long_rows() {
-    std::vector<uint64_t> rp(nl + 1);
-    GL_CUDA(cudaMemcpy(rp.data(), vf->rp, sizeof(uint64_t) * (nl + 1), cudaMemcpyDeviceToHost));
-    std::vector<uint64_t> b, e;
-    std::vector<uint32_t> rows, off(1, 0);
-    for (uint32_t r = 0; r < nl; ++r) {
-      if (rp[r + 1] - rp[r] <= kVcChunk) continue;
-      for (uint64_t c = rp[r]; c < rp[r + 1]; c += kVcChunk) {
-        b.push_back(c);
-        e.push_back(std::min<uint64_t>(c + kVcChunk, rp[r + 1]));
-      }
-      rows.push_back(r);
-      off.push_back((uint32_t) b.size());
-    }
-    nitems = (uint32_t) b.size();
-    nlong = (uint32_t) rows.size();
-    if (!nlong) return GL_OK;
-    GL_CUDA(cb.alloc(nitems));
-    GL_CUDA(ce.alloc(nitems));
-    GL_CUDA(csum.alloc(nitems));
-    GL_CUDA(lrows.alloc(nlong));
-    GL_CUDA(loff.alloc(nlong + 1));
-    GL_CUDA(cudaMemcpy(cb, b.data(), sizeof(uint64_t) * nitems, cudaMemcpyHostToDevice));
-    GL_CUDA(cudaMemcpy(ce, e.data(), sizeof(uint64_t) * nitems, cudaMemcpyHostToDevice));
-    GL_CUDA(cudaMemcpy(lrows, rows.data(), sizeof(uint32_t) * nlong, cudaMemcpyHostToDevice));
-    GL_CUDA(cudaMemcpy(loff, off.data(), sizeof(uint32_t) * (nlong + 1), cudaMemcpyHostToDevice));
-    return GL_OK;
   }
 
   int plan_gather_scatter() {
@@ -341,10 +275,10 @@ struct PageRankVcApp : gl_app {
       if (!gp) gp = persistent_grid(k_vc_pull, eng.sm_count);
       const int grid = (int) std::min<uint64_t>((uint64_t) gp, ((uint64_t) nl + kTB - 1) / kTB);
       GL_LAUNCH(k_vc_pull, grid, kTB, s, vf->rp, vf->col, nl, curr, next);
-      if (nlong) {
-        const int g2 = (int) std::min<uint64_t>((uint64_t) gp, ((uint64_t) nitems * 32 + kTB - 1) / kTB);
-        GL_LAUNCH(k_vc_chunks, g2, kTB, s, cb, ce, nitems, vf->col, curr, csum);
-        GL_LAUNCH(k_vc_long, (nlong + 255) / 256, 256, s, lrows, loff, nlong, csum, next);
+      if (lr.nlong) {
+        const int g2 = (int) std::min<uint64_t>((uint64_t) gp, ((uint64_t) lr.nitems * 32 + kTB - 1) / kTB);
+        GL_LAUNCH(k_vc_chunks, g2, kTB, s, lr.cb, lr.ce, lr.nitems, vf->col, curr, lr.csum);
+        GL_LAUNCH(k_vc_long, (lr.nlong + 255) / 256, 256, s, lr.rows, lr.off, lr.nlong, lr.csum, next);
       }
     }
     const bool last = step == cfg.max_round;
