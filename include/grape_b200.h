@@ -423,9 +423,11 @@ typedef enum {
                                result: double per master vertex, see below      */
   GL_APP_CDLP_DIRECTED = 13, /* cuda/cdlp/cdlp.h on kBothOutIn (--directed)
                                result: int64 label, see below                   */
-  GL_APP_PAGERANK_DIRECTED = 14 /* pagerank/pagerank_directed.h (PageRankDirected,
+  GL_APP_PAGERANK_DIRECTED = 14, /* pagerank/pagerank_directed.h (PageRankDirected,
                                    run_app_opt --application pagerank --directed)
                                    result: double, see below                    */
+  GL_APP_BC_SOURCES = 15 /* bc (--bc_source) summed over a list of sources set by
+                            gl_app_set_sources  result: double, see below       */
 } gl_app_kind;
 
 /* ------------------------------------------------------------------ *
@@ -601,6 +603,46 @@ typedef struct {
   int64_t depth;
 } gl_bc_value;
 
+/* GL_APP_BC_SOURCES: betweenness centrality summed over a list of sources: exact Brandes BC when the
+ * list is every vertex, the sampled approximation when it is a sample.  One double per inner vertex in
+ * lid order (gl_app_result_oids gives the oids).  A directed fragment is refused at gl_app_create with
+ * GL_ERR_ARG, as for GL_APP_BC; edge data is ignored.  The list is set by gl_app_set_sources (below)
+ * and a query before the first gl_app_set_sources returns GL_ERR_ARG.  reserved[0] is the batch width
+ * B, 1..32 (0: the largest that fits, at most 32; GL_ERR_ARG outside 0..32); with reserved[0] = 0,
+ * reserved[1] > 0 is a test hook that stands in for the batch width free HBM allows (GL_ERR_ARG when
+ * negative); every other config field is ignored.  The graph is GL_APP_BC's CSR: a multi-edge once per copy, a self loop twice.  For each entry
+ * s of the list, in list order:
+ *   depth_s and sigma_s follow GL_APP_BC's rules exactly (a depth-1 vertex has sigma 1 however many
+ *   parallel edges join it to s);
+ *   backward, from the deepest level up: cacc = the sum of t_s(w) over the entries (v, w) of v's row
+ *   with depth_s(w) = depth_s(v) + 1, in row order; delta_s(v) = cacc * sigma_s(v);
+ *   t_s(v) = (1.0 / sigma_s(v)) * (1.0 + delta_s(v)); all f64.  delta_s(v) = 0 when v = s, when v is
+ *   unreached and when s is not in the graph.
+ *   bc(v) = (((0.0 + delta_s1(v)) + delta_s2(v)) + ...), a left fold in list order.
+ * No normalisation: over every vertex of an undirected graph, bc is twice networkx's
+ * betweenness_centrality(G, normalized=False) (each pair is counted from both ends); for a sample of k
+ * of n sources the caller scales by n / k.  f32(delta_s(v)) agrees with GL_APP_BC's c (source s, v != s)
+ * within 1e-5 relative; GL_APP_BC rounds c and t to f32 at every level, this app does not.
+ * Sources run in batches of B, one warp lane per source, with every per-vertex state B lanes wide
+ * (20 B bytes per vertex); a row's sum is sequential up to 1024 entries, and a longer row is cut into
+ * 1024-entry chunks whose sums are added in chunk order.  One fragment therefore gives bit-identical
+ * output on every run and for every B.  gl_app_create returns GL_ERR_NOMEM only when B = 1 does not fit.
+ * On several fragments B is decided once for the group: the smallest width any rank's free HBM and
+ * mirror area allow, so every rank cuts the list into the same batches.
+ * Stats, one fragment: supersteps = batches; step i = batch i, mode 2, step_frontier = the vertices its
+ * sources reach (each source included; saturated at UINT32_MAX, which B sources reaching more than
+ * 2^32 / B vertices each can pass), step_entries = row entries read by its gathers;
+ * frontier_vertices = that sum over the whole list; touched_vertices = frontier_vertices minus the
+ * list entries found in the graph; entries_scanned = row entries read by the gathers (a device count).
+ * Several fragments: every rank passes the same list (checked by an all-reduce of its length and hash:
+ * GL_ERR_ARG otherwise); the row order is the fragment's own, so results agree with one fragment up to
+ * f64 summation order, and are bit-identical for every B within one grouping.  One worker round per
+ * forward level of each batch (the last one finds nothing) and one per backward level >= 1;
+ * step_frontier = this fragment's share (saturated at UINT32_MAX) of the (vertex, source) pairs of
+ * the level the round finds or processes; frontier_vertices and touched_vertices are this fragment's shares of the one-fragment
+ * values.  B is clamped to what the communicator's mirror_bytes holds for the B-wide rows of the
+ * outer copies; gl_app_create returns GL_ERR_ARG when B = 1 does not fit. */
+
 /* GL_APP_KCLIQUE: k = max_round, 3 <= k <= GL_KCLIQUE_MAX_K; a smaller or larger k and a directed
  * fragment are refused at gl_app_create with GL_ERR_ARG.  The result is ONE int64 (gl_app_result takes
  * bytes >= 8): the number of k-cliques of the whole fragment group, the same value on every rank.
@@ -638,6 +680,8 @@ typedef struct {
                             0 = one superstep per host round                    */
   int reserved[8];       /* tuning / test hooks, 0 = default:
                             [0] 1: WCC dense rounds as pull sweeps
+                                GL_APP_BC_SOURCES: the batch width B, 1..32
+                            [1] GL_APP_BC_SOURCES: the batch width free HBM is taken to allow
                             [1] 1: BFS without the hub-first shadow CSR; 2: with it also on a
                                    small graph (default: from 2^16 vertices on); 3: like 2, several
                                    fragments, without the delegated-hub lists (A/B)
@@ -717,7 +761,7 @@ int gl_vc_app_create(gl_app_t** out, int kind, gl_vcfrag_t* frag, gl_comm_t* com
  *   wcc_opt, one fragment: everything happens in PEval and is reported as step 0: step_frontier =
  *     ivnum, step_entries = entries_scanned = 2 sampled entries per vertex + the rows scanned outside
  *     the largest sampled component (which depends on the sampling's races); touched_vertices = ivnum.
- *   BC, k-clique: see gl_bc_value and GL_KCLIQUE_MAX_K above. */
+ *   BC, k-clique: see gl_bc_value and GL_KCLIQUE_MAX_K above; BC_SOURCES: see GL_APP_BC_SOURCES. */
 #define GL_MAX_STEP_STATS 512
 typedef struct {
   int supersteps;            /* rounds executed (PEval counts as round 0)      */
@@ -751,6 +795,11 @@ int gl_app_result(gl_app_t*, void* host_out, size_t bytes);
  * contiguous-block builders, where gid -> oid is arithmetic or the fragment's
  * own oid list).  The map is borrowed: keep it alive while the app is used. */
 int gl_app_set_vertex_map(gl_app_t*, const gl_vm_t* vm);
+/* GL_APP_BC_SOURCES only (any other kind: GL_ERR_ARG): copies the source list, which stays in force for
+ * later queries until it is set again.  oids == NULL with n == 0: every vertex of the fragment group, in
+ * gid order; a non-NULL list with n == 0 is the empty list (every result 0.0).  Duplicates count once
+ * per occurrence; an oid that is not a vertex contributes nothing.  Collective on a fragment group. */
+int gl_app_set_sources(gl_app_t*, const int64_t* oids, uint64_t n);
 /* oid of each inner vertex (first column of Output) */
 int gl_app_result_oids(gl_app_t*, int64_t* host_out, size_t count);
 void gl_app_destroy(gl_app_t*);

@@ -12,12 +12,12 @@ GL_LB = {"none": 0, "cm": 1, "wm": 2, "cta": 3, "strict": 4, "cmold": 5}
 APP = {"bfs": 0, "sssp": 1, "wcc": 2, "pagerank": 3, "cdlp": 4, "lcc": 5, "wcc_opt": 6,
        "core_decomposition": 7, "kcore": 8, "kclique": 9, "bc": 10,
        "lcc_directed": 11, "pagerank_vc": 12, "cdlp_directed": 13,
-       "pagerank_directed": 14}
+       "pagerank_directed": 14, "bc_sources": 15}
 # gl_bc_value: the reference's Output() line `oid c sigma depth` (c is an f32 value, widened exactly)
 BC_DTYPE = np.dtype([("centrality", "<f8"), ("path_num", "<f8"), ("depth", "<i8")])
 RESULT_DTYPE = {0: np.int64, 1: np.float64, 2: np.int64, 3: np.float64, 4: np.int64, 5: np.float64, 6: np.int64,
                 7: np.int64, 8: np.int64, 9: np.int64, 10: BC_DTYPE, 11: np.float64, 12: np.float64,
-                13: np.int64, 14: np.float64}
+                13: np.int64, 14: np.float64, 15: np.float64}
 GL_MAX_STEP_STATS = 512
 GL_IPC_HANDLE_BYTES = 64
 
@@ -111,7 +111,7 @@ SYMBOLS = [
     "gl_bitmap_clear", "gl_bitmap_count", "gl_bitmap_destroy", "gl_frag_prepare", "gl_queue_create", "gl_queue_clear",
     "gl_queue_size", "gl_queue_data", "gl_queue_fill_from_bitmap", "gl_queue_destroy", "gl_varray_create",
     "gl_varray_h2d", "gl_varray_d2h", "gl_varray_destroy", "gl_app_config_default", "gl_app_create", "gl_app_query", "gl_app_result",
-    "gl_app_result_oids", "gl_app_destroy", "gl_edge_scan_queue", "gl_compact_bitmap", "gl_dev_alloc",
+    "gl_app_result_oids", "gl_app_set_sources", "gl_app_destroy", "gl_edge_scan_queue", "gl_compact_bitmap", "gl_dev_alloc",
     "gl_dev_free", "gl_dev_memset", "gl_dev_h2d", "gl_dev_d2h", "gl_dev_sync", "gl_kernel_launch_count",
     "gl_host_alloc_pinned", "gl_host_free_pinned", "gl_vcfrag_create", "gl_vcfrag_build_rmat",
     "gl_vcfrag_get_info", "gl_vcfrag_destroy", "gl_vc_app_create",
@@ -514,10 +514,14 @@ class App:
     default.  The result of "kclique" is one Python int: the k-clique count of the
     whole fragment group (result() takes no out array for it).  "bc" takes its
     source as App("bc", frag, source_oid=...) and returns a BC_DTYPE record
-    (centrality, path_num, depth) per inner vertex.  A VcFragment takes "pagerank_vc"
-    (gl_vc_app_create); its result is one double per master vertex."""
+    (centrality, path_num, depth) per inner vertex.  "bc_sources" takes its list as
+    App("bc_sources", frag, sources=[oids] or None (every vertex)) or later through
+    set_sources(); its result is one double per inner vertex.  A VcFragment takes
+    "pagerank_vc" (gl_vc_app_create); its result is one double per master vertex."""
 
-    def __init__(self, kind, frag, comm=None, **cfg):
+    _NO_LIST = object()
+
+    def __init__(self, kind, frag, comm=None, sources=_NO_LIST, **cfg):
         self.kind = APP[kind] if isinstance(kind, str) else kind
         self.frag = frag
         if self.kind in (APP["kcore"], APP["kclique"]):
@@ -542,6 +546,17 @@ class App:
         create = lib().gl_vc_app_create if isinstance(frag, VcFragment) else lib().gl_app_create
         check(create(C.byref(self.h), self.kind, frag.h, comm.h if comm else None, C.byref(c)))
         self.stats = QueryStats()
+        if sources is not App._NO_LIST:
+            self.set_sources(sources)
+
+    def set_sources(self, oids):
+        """gl_app_set_sources: the list of source oids (None: every vertex of the fragment group)."""
+        if oids is None:
+            check(lib().gl_app_set_sources(self.h, None, C.c_uint64(0)))
+            return
+        self._sources = np.ascontiguousarray(oids, dtype=np.int64)
+        check(lib().gl_app_set_sources(self.h, self._sources.ctypes.data_as(C.c_void_p),
+                                       C.c_uint64(len(self._sources))))
 
     def set_vertex_map(self, vm):
         self._vm = vm

@@ -85,6 +85,7 @@ struct gl_app {
   virtual int ResultOids(int64_t* host_out, size_t count);               // gl_app_result_oids (worker.cu)
   virtual void FillStats(gl_query_stats*) {}   // apps that time supersteps on the device
   virtual void AfterRound() {}                 // runs after every FinishARound (global round statistics)
+  virtual int SetSources(const int64_t*, uint64_t);                      // gl_app_set_sources (worker.cu)
   // Apps whose whole query is one launch record this event in-stream right after the query's last
   // device operation (kernel + control-block read-back); query_ms then ends there instead of at the
   // event the host records after it woke up from the stream synchronisation (host latency is part of
@@ -126,5 +127,6 @@ gl_app* make_core_decomposition();
 gl_app* make_kcore();
 gl_app* make_kclique();
 gl_app* make_bc();
+gl_app* make_bc_sources();
 gl_app* make_pagerank_vc(gl_vcfrag* f);
 }  // namespace gl

@@ -237,6 +237,23 @@ __global__ void k_mirror_unpack_vals(T* values, const uint32_t* __restrict__ gho
   for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x)
     values[base + k] = in[k];
 }
+// rows of w 8-byte words: one thread per word
+__global__ void k_mirror_pack_rows(const uint64_t* __restrict__ values, uint32_t w, const uint32_t* __restrict__ lids,
+                                   const uint64_t* __restrict__ off, char* const* msend) {
+  const uint32_t g = blockIdx.y;
+  const uint64_t b = off[g], n = (off[g + 1] - b) * w;
+  uint64_t* out = (uint64_t*) msend[g];
+  for (uint64_t k = (uint64_t) blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (uint64_t) gridDim.x * blockDim.x)
+    out[k] = values[(uint64_t) lids[b + k / w] * w + k % w];
+}
+__global__ void k_mirror_unpack_rows(uint64_t* values, uint32_t w, const uint32_t* __restrict__ ghost_range,
+                                     const char* const* mrecv) {
+  const uint32_t f = blockIdx.y;
+  const uint64_t base = (uint64_t) ghost_range[f] * w, n = (uint64_t) (ghost_range[f + 1] - ghost_range[f]) * w;
+  const uint64_t* in = (const uint64_t*) mrecv[f];
+  for (uint64_t k = (uint64_t) blockIdx.x * blockDim.x + threadIdx.x; k < n; k += (uint64_t) gridDim.x * blockDim.x)
+    values[base + k] = in[k];
+}
 }  // namespace
 
 int MessageManager::PeerBarrier(cudaStream_t s) {
@@ -432,6 +449,37 @@ int MessageManager::SyncValuesToGhosts(cudaStream_t s, void* values, int elem_by
   return GL_OK;
 }
 
+size_t MessageManager::MaxRowBytes() const {
+  if (fnum == 1) return SIZE_MAX;
+  uint32_t most = 0;
+  for (uint32_t f = 0; f < fnum; ++f) most = std::max(most, ghost_range[f + 1] - ghost_range[f]);
+  return most ? comm->mirror_bytes / most : SIZE_MAX;
+}
+
+int MessageManager::SyncRowsToGhosts(cudaStream_t s, void* values, int row_bytes) {
+  if (fnum == 1) return GL_OK;
+  if (row_bytes <= 0 || row_bytes % 8 || row_bytes > 256 || (size_t) row_bytes > MaxRowBytes()) {
+    set_error("SyncRowsToGhosts: %d-byte rows do not fit the mirror-sync area (%zu bytes per peer)", row_bytes,
+              comm->mirror_bytes);
+    return GL_ERR_ARG;
+  }
+  const uint32_t w = (uint32_t) row_bytes / 8;
+  comm->mirror_dirty = true;
+  const int par = (int) (++mirror_seq & 1);
+  dim3 grid(num_sms() * 8, fnum);
+  if (mirror_total) {
+    k_mirror_pack_rows<<<grid, 256, 0, s>>>((const uint64_t*) values, w, d_mirror_lids, d_mirror_off, d_msend[par]);
+    GL_COUNT_LAUNCH();
+    GL_CUDA(cudaGetLastError());
+  }
+  GL_TRY(PeerBarrierAsync(s));
+  if (ghost_range[fnum] > ghost_range[0]) {
+    k_mirror_unpack_rows<<<grid, 256, 0, s>>>((uint64_t*) values, w, d_ghost_range, d_mrecv[par]);
+    GL_COUNT_LAUNCH();
+    GL_CUDA(cudaGetLastError());
+  }
+  return GL_OK;
+}
 
 int MessageManager::PeerAllReduce(cudaStream_t s, long long* i0, long long* i1, double* d0, int op) {
   const unsigned long long tag = ++comm->seq_base;

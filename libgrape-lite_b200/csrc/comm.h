@@ -144,6 +144,11 @@ struct MessageManager {
   bool has_mirror_plan() const { return d_mirror_lids != nullptr || mirror_total == 0 && plan_built; }
   int SyncBitsToGhosts(cudaStream_t s, uint32_t* bitmap);   // ghost bits |= owner bits
   int SyncValuesToGhosts(cudaStream_t s, void* values, int elem_bytes);  // values[ghost] = owner value
+  // the same for rows of row_bytes (a multiple of 8, up to 256): values[ghost * row_bytes ..] = owner's row;
+  // GL_ERR_ARG when one peer's outer copies do not fit mirror_bytes (see MaxRowBytes)
+  int SyncRowsToGhosts(cudaStream_t s, void* values, int row_bytes);
+  // the largest row the mirror area holds for every peer's outer copies (after BuildMirrorPlan)
+  size_t MaxRowBytes() const;
   bool plan_built = false;
   uint32_t plan_ivnum = 0;
   DevBuf<uint32_t> d_mirror_lids;          // my inner lids mirrored elsewhere, grouped by holder

@@ -124,6 +124,7 @@ int gl_app_create(gl_app_t** out, int kind, gl_frag_t* frag, gl_comm_t* comm,
     case GL_APP_KCORE: a = make_kcore(); break;
     case GL_APP_KCLIQUE: a = make_kclique(); break;
     case GL_APP_BC: a = make_bc(); break;
+    case GL_APP_BC_SOURCES: a = make_bc_sources(); break;
     case GL_APP_LCC_DIRECTED: a = make_lcc_directed(); break;
     case GL_APP_CDLP_DIRECTED: a = make_cdlp_directed(); break;
     case GL_APP_PAGERANK_DIRECTED: a = make_pagerank_directed(); break;
@@ -259,12 +260,23 @@ int gl_app_result(gl_app_t* a, void* host_out, size_t bytes) {
   return a->Result(host_out, bytes);
 }
 
+int gl_app_set_sources(gl_app_t* a, const int64_t* oids, uint64_t n) {
+  GL_ARG(a, "null argument");
+  GL_ARG(oids || n == 0, "gl_app_set_sources: a NULL list must have n = 0");
+  return a->SetSources(oids, n);
+}
+
 int gl_app_result_oids(gl_app_t* a, int64_t* host_out, size_t count) {
   GL_ARG(a && host_out, "null argument");
   return a->ResultOids(host_out, count);
 }
 
 }  // extern "C"
+
+int gl_app::SetSources(const int64_t*, uint64_t) {
+  set_error("gl_app_set_sources: app kind %d takes no source list (GL_APP_BC_SOURCES only)", kind);
+  return GL_ERR_ARG;
+}
 
 int gl_app::ResultOids(int64_t* host_out, size_t count) {
   GL_ARG(count >= frag->ivnum, "bad argument");
