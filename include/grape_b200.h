@@ -426,8 +426,11 @@ typedef enum {
   GL_APP_PAGERANK_DIRECTED = 14, /* pagerank/pagerank_directed.h (PageRankDirected,
                                    run_app_opt --application pagerank --directed)
                                    result: double, see below                    */
-  GL_APP_BC_SOURCES = 15 /* bc (--bc_source) summed over a list of sources set by
-                            gl_app_set_sources  result: double, see below       */
+  GL_APP_BC_SOURCES = 15, /* bc (--bc_source) summed over a list of sources set by
+                             gl_app_set_sources  result: double, see below      */
+  GL_APP_PAGERANK_LOCAL = 16 /* pagerank/pagerank_local.h (PageRankLocal, run_app
+                                --application pagerank_local): un-normalised
+                                PageRank  result: double, see below             */
 } gl_app_kind;
 
 /* ------------------------------------------------------------------ *
@@ -574,6 +577,33 @@ void gl_vcfrag_destroy(gl_vcfrag_t*);
  *   by the other fragments (the dense mirror sync of x after PEval and after rounds 1..R-1) and 8 (F - 1)
  *   is the value S this fragment sends to its peers in each all-reduce after rounds 1..R-1.
  *   R <= 0: 0. */
+
+/* GL_APP_PAGERANK_LOCAL: the original, un-normalised PageRank (the reference's PageRankLocal, run_app
+ * --application pagerank_local), one double per inner vertex in lid order.  The ranks sum to about N
+ * rather than 1, and no dangling mass is redistributed.  Undirected and directed fragments are both
+ * accepted; on a directed one the sum runs over the out-row (the reference's kOnlyOut), so ie is not
+ * needed.  Uses pr_delta (d) and max_round (R); every other gl_app_config field, pr_pull included, is
+ * ignored; edge data is ignored.  deg(v) = the entries of v's out-row (a multi-edge counts once per
+ * copy, a self loop as often as the fragment stores it: twice on an undirected fragment, once on a
+ * directed one).
+ *   R <= 0 is refused at gl_app_create with GL_ERR_ARG (the reference never terminates there).
+ *   PEval: x(v) = 1 / deg(v), or 1 when deg(v) = 0.
+ *   Round k = 1..R: c(v) = (1 - d) + d * (sum of x(u) over the entries u of v's out-row);
+ *          k < R: x(v) = c(v) / deg(v), or c(v) when deg(v) = 0.
+ *   Output: c(v) of round R (not divided).
+ * On an undirected fragment with no zero-degree vertex the result equals N x GL_APP_PAGERANK (same d and
+ * R) in real arithmetic; with zero-degree vertices the two are not related by a scale factor.  The
+ * reference's single-fragment run on a graph whose average out-row length exceeds 10 never divides by
+ * the degree after PEval (its values grow every round); this app follows the definition above on any
+ * number of fragments.
+ * Everything is f64, and every sum has a fixed order: an out-row in the row tiers of GL_APP_PAGERANK_VC
+ * (a thread up to 32 entries, a warp up to 4096, longer rows in 4096-entry chunks folded in order).  The
+ * same input on the same fragments gives bit-identical output on every run.
+ * Stats: supersteps = R + 1; step k = round k (1..R), mode 2, step_frontier = ivnum, step_entries = the
+ *   fragment's oe entries (a host count), so entries_scanned = R x oe entries; touched_vertices = ivnum
+ *   x R.  msg_bytes_sent (F > 1) = R x 8 M, where M = the outer copies of this fragment's inner vertices
+ *   held by the other fragments (the dense mirror sync of x after PEval and after rounds 1..R-1);
+ *   0 on one fragment. */
 
 /* GL_APP_BC: single-source betweenness centrality, one gl_bc_value per inner vertex in lid order: the
  * reference's Output() line `oid c sigma depth` (gl_app_result_oids gives the oid).  A directed fragment
@@ -740,7 +770,7 @@ int gl_vc_app_create(gl_app_t** out, int kind, gl_vcfrag_t* frag, gl_comm_t* com
  *     not counted by a kernel.
  *   CDLP_DIRECTED: as CDLP, with step_entries = the ie entries plus the oe entries of the fragment's
  *     inner rows (both gathers and sorts); supersteps = max_round + 1, touched_vertices = ivnum x rounds.
- *   PAGERANK_DIRECTED: see GL_APP_PAGERANK_DIRECTED above.
+ *   PAGERANK_DIRECTED: see GL_APP_PAGERANK_DIRECTED above; PAGERANK_LOCAL: see GL_APP_PAGERANK_LOCAL.
  *   LCC, one fragment: step 1 counts the triangles: step_frontier = ivnum, step_entries = for every
  *     entry (v, u) of the degree-ordered DAG, the length of u's DAG row; supersteps = 3.
  *   LCC_DIRECTED: step 1 counts the triangles (mode 2): step_frontier = ivnum, step_entries = for every

@@ -12,12 +12,12 @@ GL_LB = {"none": 0, "cm": 1, "wm": 2, "cta": 3, "strict": 4, "cmold": 5}
 APP = {"bfs": 0, "sssp": 1, "wcc": 2, "pagerank": 3, "cdlp": 4, "lcc": 5, "wcc_opt": 6,
        "core_decomposition": 7, "kcore": 8, "kclique": 9, "bc": 10,
        "lcc_directed": 11, "pagerank_vc": 12, "cdlp_directed": 13,
-       "pagerank_directed": 14, "bc_sources": 15}
+       "pagerank_directed": 14, "bc_sources": 15, "pagerank_local": 16}
 # gl_bc_value: the reference's Output() line `oid c sigma depth` (c is an f32 value, widened exactly)
 BC_DTYPE = np.dtype([("centrality", "<f8"), ("path_num", "<f8"), ("depth", "<i8")])
 RESULT_DTYPE = {0: np.int64, 1: np.float64, 2: np.int64, 3: np.float64, 4: np.int64, 5: np.float64, 6: np.int64,
                 7: np.int64, 8: np.int64, 9: np.int64, 10: BC_DTYPE, 11: np.float64, 12: np.float64,
-                13: np.int64, 14: np.float64, 15: np.float64}
+                13: np.int64, 14: np.float64, 15: np.float64, 16: np.float64}
 GL_MAX_STEP_STATS = 512
 GL_IPC_HANDLE_BYTES = 64
 

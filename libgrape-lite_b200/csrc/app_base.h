@@ -118,6 +118,7 @@ gl_app* make_sssp_f64();
 gl_app* make_wcc();
 gl_app* make_pagerank();
 gl_app* make_pagerank_directed();
+gl_app* make_pagerank_local();
 gl_app* make_cdlp();
 gl_app* make_cdlp_directed();
 gl_app* make_lcc();

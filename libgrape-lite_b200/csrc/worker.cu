@@ -128,6 +128,7 @@ int gl_app_create(gl_app_t** out, int kind, gl_frag_t* frag, gl_comm_t* comm,
     case GL_APP_LCC_DIRECTED: a = make_lcc_directed(); break;
     case GL_APP_CDLP_DIRECTED: a = make_cdlp_directed(); break;
     case GL_APP_PAGERANK_DIRECTED: a = make_pagerank_directed(); break;
+    case GL_APP_PAGERANK_LOCAL: a = make_pagerank_local(); break;
     case GL_APP_PAGERANK_VC:
       set_error("GL_APP_PAGERANK_VC runs on a vertex-cut fragment: use gl_vc_app_create");
       return GL_ERR_ARG;
