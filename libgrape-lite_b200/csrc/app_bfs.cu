@@ -338,6 +338,13 @@ struct PullArgs {
   uint32_t list_cap;
 };
 
+// A thread's share of a pull level's entries scanned and vertices expanded, when the caller adds them
+// with the CTA's other counters (flush_acc_cta) instead of the phase adding them per warp.
+struct PullCounts {
+  unsigned long long scanned = 0;
+  uint32_t frontier = 0;
+};
+
 // is vertex `id` in the frontier?  kGlobal is a compile-time switch: the single-fragment kernels
 // keep the plain local-bitmap probe (a run-time branch here cost 8 % of the whole query)
 template <bool kGlobal>
@@ -385,11 +392,13 @@ GL_DEV uint32_t pull_probe_nibble(const PullArgs& a, const uint32_t* __restrict_
 // word with plain stores (the word belongs to this thread during the pull).
 // kTail (single-fragment fused kernel): the PullArgs hub_first fields apply,
 // and make_list appends the candidates left unresolved to a.list, counted in
-// ctrl->aux_ticket (the level that starts the tail, see bfs_list_pull).
+// ctrl->aux_ticket (the level that starts the tail, see bfs_list_pull), and
+// the level's scanned / frontier counts are left in *cnt for the caller.
 template <bool kGlobal, bool kTail = false>
 GL_DEV bool bfs_pull_phase(PullSmem& sm, const PullArgs& a,
                            const uint32_t* __restrict__ cur, uint32_t* vis,
-                           uint32_t* nxt, ScanCtrl* ctrl, ScanAcc& acc, bool make_list = false) {
+                           uint32_t* nxt, ScanCtrl* ctrl, ScanAcc& acc, bool make_list = false,
+                           PullCounts* cnt = nullptr) {
   const uint32_t nwords = (a.ivnum + 31) / 32;
   const bool hub_first = kTail && a.hub_first;
   // hub-first order: entry 0 of a row is hub_nbr[v], which stage 1 has just tested
@@ -598,6 +607,11 @@ GL_DEV bool bfs_pull_phase(PullSmem& sm, const PullArgs& a,
       if (sm.stage_base + i < a.list_cap) a.list[sm.stage_base + i] = sm.stage[i];
   }
   acc.touched = acc.next_count;
+  if (kTail) {
+    cnt->scanned = scanned;
+    cnt->frontier = cand;
+    return shipped;
+  }
   unsigned long long s = warp_sum((unsigned long long) scanned);
   if (lane_id() == 0 && s) atomicAdd(&ctrl->scanned, s);
   if (threadIdx.x == 0 && cand) atomicAdd(&ctrl->frontier, (unsigned long long) cand);
@@ -622,8 +636,9 @@ k_bfs_pull(PullArgs a, const uint32_t* __restrict__ cur, uint32_t* vis,
 // with atomicOr.  A resolved entry is overwritten with kInfU32 in place: the
 // list is not compacted (no atomic round trip per level; in the tail few
 // entries resolve per level, and a dead entry costs one coalesced load).
+// The level's counts are left in `cnt` for flush_acc_cta.
 GL_DEV void bfs_list_pull(const PullArgs& a, const uint32_t* __restrict__ cur, uint32_t* vis, uint32_t* nxt,
-                          uint32_t n, ScanCtrl* ctrl, ScanAcc& acc) {
+                          uint32_t n, ScanAcc& acc, PullCounts& cnt) {
   uint32_t* list = a.list;
   const uint32_t lane = lane_id();
   uint64_t scanned = 0;
@@ -672,10 +687,8 @@ GL_DEV void bfs_list_pull(const PullArgs& a, const uint32_t* __restrict__ cur, u
     }
   }
   acc.touched = acc.next_count;
-  const unsigned long long s = warp_sum((unsigned long long) scanned);
-  const uint32_t c = warp_sum(cand);
-  if (lane == 0 && s) atomicAdd(&ctrl->scanned, s);
-  if (lane == 0 && c) atomicAdd(&ctrl->frontier, (unsigned long long) c);
+  cnt.scanned = scanned;
+  cnt.frontier = cand;
 }
 
 // ---------------------------------------------------------------------------
@@ -718,7 +731,8 @@ struct BfsFusedCtl {
   unsigned long long xw[32][2];  // GL_TRACE: per level: peer wait / first grid.sync of its last xsync
   unsigned long long l_nf;               // several fragments: this fragment's part of the current frontier (statistics)
   unsigned long long r_visited_cnt_g;    // several fragments: vertices visited so far in the whole graph (resume state)
-  unsigned long long t_kstart, t_kend;   // GL_TRACE: first / last instruction of the fused multi-fragment kernel (thread 0)
+  // thread 0's first instruction of the fused multi-fragment kernel / last of either fused kernel (GL_KTIME)
+  unsigned long long t_kstart, t_kend;
   unsigned long long xt[8];      // GL_TRACE: timestamps inside the most recent xsync (block 0, thread 0)
   uint32_t x_error, x_pad;   // 1 = a peer did not show up in time, 2 = landing slot overflow
   BfsLevelStat stat[kMaxFusedStats];
@@ -945,34 +959,30 @@ GL_DEV void bfs_source_row_push(const EdgeRange& er, const OpBfsPush& op, uint32
   }
 }
 
-// flush_acc for a phase after which every warp of the grid holds counts (bfs_source_row_push): the
-// CTA sums them first and adds them with one atomic per counter: with an atomic per warp and
-// counter (flush_acc), level 0 took 7 us longer on an H100 at 700 W.  Leaves `acc` empty.
+// flush_acc for a phase after which every warp of the grid holds counts (bfs_source_row_push, the
+// pull levels of k_bfs_fused): the CTA sums them first and adds them with one atomic per counter:
+// with an atomic per warp and counter (flush_acc), level 0 took 7 us longer on an H100 at 700 W.
+// `pc` carries a pull level's scanned / frontier counts.  Leaves `acc` empty.
 struct AccSmem {
-  unsigned long long v[5][kTB / 32];
+  unsigned long long v[7][kTB / 32];
 };
-GL_DEV void flush_acc_cta(ScanAcc& acc, ScanCtrl* c, AccSmem& sm) {
-  static_assert(offsetof(ScanCtrl, touched) - offsetof(ScanCtrl, next_count) == 4 * sizeof(unsigned long long),
-                "next_count, next_edges, remote_count, aux, touched are consecutive");
+GL_DEV void flush_acc_cta(ScanAcc& acc, ScanCtrl* c, AccSmem& sm, const PullCounts& pc = PullCounts()) {
+  static_assert(offsetof(ScanCtrl, touched) - offsetof(ScanCtrl, scanned) == 6 * sizeof(unsigned long long),
+                "scanned, frontier, next_count, next_edges, remote_count, aux, touched are consecutive");
   const uint32_t wid = threadIdx.x >> 5;
-  const unsigned long long s0 = warp_sum((unsigned long long) acc.next_count);
-  const unsigned long long s1 = warp_sum((unsigned long long) acc.next_edges);
-  const unsigned long long s2 = warp_sum((unsigned long long) acc.remote);
-  const unsigned long long s3 = warp_sum((unsigned long long) acc.aux);
-  const unsigned long long s4 = warp_sum((unsigned long long) acc.touched);
-  if (lane_id() == 0) {
-    sm.v[0][wid] = s0;
-    sm.v[1][wid] = s1;
-    sm.v[2][wid] = s2;
-    sm.v[3][wid] = s3;
-    sm.v[4][wid] = s4;
+  const unsigned long long x[7] = {pc.scanned, pc.frontier, acc.next_count, acc.next_edges, acc.remote, acc.aux,
+                                   acc.touched};
+#pragma unroll
+  for (int k = 0; k < 7; ++k) {
+    const unsigned long long s = warp_sum(x[k]);
+    if (lane_id() == 0) sm.v[k][wid] = s;
   }
   __syncthreads();
-  if (threadIdx.x < 5) {
+  if (threadIdx.x < 7) {
     unsigned long long s = 0;
 #pragma unroll
     for (int w = 0; w < kTB / 32; ++w) s += sm.v[threadIdx.x][w];
-    if (s) atomicAdd(&c->next_count + threadIdx.x, s);
+    if (s) atomicAdd(&c->scanned + threadIdx.x, s);
   }
   acc = ScanAcc();
 }
@@ -994,16 +1004,17 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
   __shared__ uint32_t s_item;
   BfsFusedCtl* ctl = a.ctl;
   const uint32_t gtid = blockIdx.x * blockDim.x + threadIdx.x;
-  // running totals, replicated in every thread
-  unsigned long long n_f, m_f, visited_edges, visited_cnt;
+  // running totals, replicated in every thread (the frontier's edges m_f are not kept: only the
+  // phase rule reads them, right after a level, and a park reads them back from the counters)
+  unsigned long long n_f, visited_edges, visited_cnt;
   const unsigned long long m_total = a.m_total;   // a kernel parameter: no register held across the levels
   uint32_t phase;
   if (a.depth_base == 0) {
     // first launch: the query starts here, with the source as the frontier of level 0
     const unsigned long long deg = a.has_src ? a.er.rp[a.src + 1] - a.er.rp[a.src] : 0ull;
     n_f = visited_cnt = a.has_src ? 1ull : 0ull;
-    m_f = visited_edges = deg;
-    phase = bfs_next_phase(0, n_f, m_f, m_total - visited_edges, a.pa.ivnum, a.direction_opt, a.beta, a.nz_total,
+    visited_edges = deg;
+    phase = bfs_next_phase(0, n_f, deg, m_total - visited_edges, a.pa.ivnum, a.direction_opt, a.beta, a.nz_total,
                            kTailPerFrontier);
     if (gtid == 0) {
       ctl->t_begin = global_ns();
@@ -1017,14 +1028,19 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
     if (phase != 0) grid.sync();
   } else {
     n_f = ctl->r_nf;
-    m_f = ctl->r_mf;
     visited_edges = ctl->r_visited_edges;
     visited_cnt = ctl->r_visited_cnt;
     phase = ctl->r_phase;
   }
   for (uint32_t depth = 0; n_f != 0; ++depth) {
     if (depth + 1 >= a.max_lv) {
-      if (gtid == 0) bfs_park(ctl, n_f, m_f, visited_edges, visited_cnt, phase);
+      if (gtid == 0) {
+        // m_f: the last level's next_edges (its counters are cleared one level later), else the launch's
+        // start value (a first launch's level 0: the source's degree = visited_edges)
+        const unsigned long long m_f = depth ? ((const volatile ScanCtrl*) &ctl->c[(depth + 2) % 3])->next_edges
+                                             : (a.depth_base ? ctl->r_mf : visited_edges);
+        bfs_park(ctl, n_f, m_f, visited_edges, visited_cnt, phase);
+      }
       break;
     }
     ScanCtrl* C = &ctl->c[depth % 3];
@@ -1039,10 +1055,15 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
     if (phase == kListPull) {
       const uint32_t n = ((const volatile ScanCtrl*) &ctl->c[(depth + 2) % 3])->aux_ticket;
       if (gtid == 0) C->aux_ticket = n;
-      bfs_list_pull(a.pa, cur, a.vis, nxt, n, C, acc);
+      PullCounts pc;
+      bfs_list_pull(a.pa, cur, a.vis, nxt, n, acc, pc);
+      flush_acc_cta(acc, C, sm.acc, pc);
     } else if (phase == 1) {
+      PullCounts pc;
       bfs_pull_phase<false, true>(sm.pull, a.pa, cur, a.vis, nxt, C, acc,
-                                  a.pa.list_cap && a.nz_total <= visited_cnt + a.list_gap);
+                                  a.pa.list_cap && a.nz_total <= visited_cnt + a.list_gap, &pc);
+      // (sm.acc overlaps only the head of sm.pull.v, which the phase does not read after its last ticket)
+      flush_acc_cta(acc, C, sm.acc, pc);
     } else {
       OpBfsPush op{a.vis, nxt, nullptr, a.er.rp, a.pa.ivnum, a.deg8};
       if (depth == 0 && a.depth_base == 0) {
@@ -1053,9 +1074,9 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
         grid.sync();
         if (a.hub_tma) hub_scan_phase_tma<OpBfsPush>(sm.hub, a.er, op, C, a.hubs, a.hub_cap, acc);
         else hub_scan_phase<OpBfsPush>(&s_item, a.er, op, C, a.hubs, a.hub_cap, acc);
+        flush_acc(acc, C);
       }
     }
-    flush_acc(acc, C);
     grid.sync();
     const volatile ScanCtrl* VC = C;
     const unsigned long long next_count = VC->next_count;
@@ -1064,17 +1085,17 @@ __global__ void __launch_bounds__(kTB, GL_BFS_FUSED_CTAS) k_bfs_fused(BfsFusedAr
                         VC->aux_ticket <= a.pa.list_cap;
     if (gtid == 0) bfs_level_end(ctl, a.depth_base, depth, n_f, (phase == 1 || phase == kListPull) ? 1u : 0u);
     n_f = next_count;
-    m_f = next_edges;
     visited_edges += next_edges;
     visited_cnt += next_count;
     // while a list is in use the level costs O(list) and one grid.sync: keep pulling (depths are the
     // same in either direction)
     phase = listed ? kListPull
-                   : bfs_next_phase(phase, n_f, m_f,
+                   : bfs_next_phase(phase, n_f, next_edges,
                                     m_total > visited_edges ? m_total - visited_edges : 0,
                                     a.pa.ivnum, a.direction_opt, a.beta,
                                     a.nz_total > visited_cnt ? a.nz_total - visited_cnt : 0, kTailPerFrontier);
   }
+  if (gtid == 0) ctl->t_kend = global_ns();
 }
 
 
@@ -2096,6 +2117,17 @@ struct BfsApp : gl_app {
     if (multi && getenv("GL_KTIME"))   // (not under GL_TRACE: its per-launch synchronisation distorts the gaps)
       fprintf(stderr, "[gl-ktime] f%u seed end -> first instruction %.1f us, kernel %.1f us, levels %u\n", fv.fid,
               (double) (h_ctl->t_kstart - h_ctl->t_begin) * 1e-3, (double) (h_ctl->t_kend - h_ctl->t_kstart) * 1e-3, h_ctl->levels);
+    if (!multi && getenv("GL_KTIME") && h_ctl->levels && h_ctl->levels <= (uint32_t) kMaxFusedStats) {
+      // one fragment: t_begin is the kernel's first instruction; what the query's events add around
+      // the kernel is the launch and the epilogue (control block copy, end event)
+      float ev_ms = 0.f;
+      GL_CUDA(cudaEventElapsedTime(&ev_ms, rec.ev[0], ev_done));
+      const unsigned long long t_last = h_ctl->stat[h_ctl->levels - 1].t_ns;
+      fprintf(stderr, "[gl-ktime] first instruction -> last level %.1f us, last level -> kernel end %.1f us, "
+              "events - kernel %.1f us, levels %u\n", (double) (t_last - h_ctl->t_begin) * 1e-3,
+              (double) (h_ctl->t_kend - t_last) * 1e-3, ev_ms * 1e3 - (double) (h_ctl->t_kend - h_ctl->t_begin) * 1e-3,
+              h_ctl->levels);
+    }
     if (multi && trace_on()) {
       for (uint32_t l = 0; l < h_ctl->levels && l < 32; ++l) {
         const unsigned long long* t = h_ctl->ph[l];
